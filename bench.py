@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the HIPIE inference hot path on B200 (contract: see the task statement / DESIGN.md §6).
+"""Benchmark of the HIPIE inference hot path on the H100 (DESIGN.md §6).
 
   python bench.py --gpus N --steps K --warmup W [--config C]          # product arm (one process per GPU under torchrun for N>1)
   python bench.py --impl reference --gpus N --steps K ... [--config C]  # reference arm: the CPU oracle of the same path, rank 0 only
+  python bench.py ... --dump-outputs DIR   # also write what the last timed step computed as DIR/<name>.npy (same inputs every run)
 
 Workloads (BASELINE.json `configs`, SURVEY.md §8d; per-GPU shards of the image-sharded global batches):
   --config 1 (default, the configuration the metric is quoted on)  ViT-H, 8 x 1024x1024, 80-class COCO vocabulary (Lt = 512), detection
@@ -98,7 +99,7 @@ def batch_text(cfg, B, seed_base=0):
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -143,7 +144,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; a power-limited card sustains less
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------------ CPU oracle arm
@@ -188,7 +190,9 @@ def run_reference(args, cfg):
         total, threads, sample = cpu_oracle_seconds_per_image(cfg, verbose=True)
         if i >= warm:
             secs.append(total)
-        if secs and time.perf_counter() - t_start + 1.2 * total > args.ref_budget_s:
+        if secs and len(secs) < args.steps and time.perf_counter() - t_start + 1.2 * total > args.ref_budget_s:
+            print(f"[reference] --ref-budget-s {args.ref_budget_s:.0f} s reached: {len(secs)} of the {args.steps} requested steps timed "
+                  "(raise --ref-budget-s to time them all)", file=sys.stderr)
             break                        # keep the whole reference run within a few minutes
     spi = sorted(secs)[len(secs) // 2]
     val = 1.0 / spi
@@ -206,19 +210,38 @@ def run_reference(args, cfg):
 
 
 # ------------------------------------------------------------------------------------------ product arm
-def ncu_traffic(kernel_tag):
-    """DRAM bytes per launch of the dominant kernel class from the committed `ncu --set full` capture of THIS round
-    (profiles/r02_ncu_summary.json, keyed by the same tags the live profiler uses); None when no capture of that class is committed."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_summary.json")
-    try:
-        d = json.load(open(p))
-        e = d.get(kernel_tag)
-        if e:
-            return e["dram_bytes_per_launch"], f"committed ncu capture profiles/r02_ncu_summary.json[{kernel_tag}] ({e.get('launch', '')}, commit {d.get('_commit', '?')}): " \
-                                               f"dram__bytes_read.sum + dram__bytes_write.sum of one launch; not re-measured in this run"
-    except Exception:
-        pass
-    return None, None
+def dump_outputs(out, dirname, budget=64 << 20, per_array=8 << 20):
+    """Writes the tensors of one step's result as dirname/<name>.npy (floating point -> float32, integers / bool -> float64).  An
+    array larger than `per_array` bytes is replaced by a fixed, seeded sample of its flat elements (indices from seed 0, sorted),
+    and arrays stop once `budget` bytes are written; names are visited in sorted order so that two runs write the same set."""
+    import numpy as np
+    import torch
+    flat = {}
+
+    def walk(prefix, v):
+        if isinstance(v, torch.Tensor):
+            flat[prefix] = v
+        elif isinstance(v, dict):
+            for k, x in v.items():
+                walk(f"{prefix}.{k}" if prefix else str(k), x)
+        elif isinstance(v, (list, tuple)):
+            for i, x in enumerate(v):
+                walk(f"{prefix}.{i}" if prefix else str(i), x)
+    walk("", out)
+    os.makedirs(dirname, exist_ok=True)
+    used = 0
+    for name in sorted(flat):
+        t = flat[name].detach()
+        dt = np.float32 if (t.is_floating_point() or t.is_complex()) else np.float64
+        a = t.float().cpu().numpy() if dt is np.float32 else t.to(torch.float64).cpu().numpy()
+        a = a.astype(dt).reshape(-1) if a.nbytes > per_array else a.astype(dt)
+        if a.nbytes > per_array:
+            n = per_array // a.itemsize
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))]
+        if used + a.nbytes > budget:
+            break
+        np.save(os.path.join(dirname, name.replace(os.sep, "_") + ".npy"), a)
+        used += a.nbytes
 
 
 def run_product(args, cfg):
@@ -306,10 +329,12 @@ def run_product(args, cfg):
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             s.record()
             for _ in range(args.steps):
-                hot_step()
+                last = hot_step()
             e.record()
             barrier()
         ms = s.elapsed_time(e)
+        if args.dump_outputs and rank == 0 and args.steps > 0:
+            dump_outputs(last, args.dump_outputs)
         launches = _lib.launch_count() - launches0
         if graphed is not None:          # replayed launches are not re-counted by the library: kernels per capture x replays
             launches = graphed.launches_per_replay * args.steps
@@ -391,7 +416,7 @@ def run_product(args, cfg):
                 "executed_tflops": g_exe, "executed_frac": g_exe / pk["tf_sustained"],
                 "classes": {t: round(v["ms"] / g_ms, 4) for t, v in sorted(gsel, key=lambda kv: -kv[1]["ms"])}}
     tk = kernels[top[0]]
-    traffic, traffic_note = ncu_traffic(top[0])
+    traffic, traffic_note = None, "not measured"
     roofline = {"kernel": top[0], "bound": tk.get("bound", "tensor"), "achieved": tk.get("achieved"),
                 "peak": pk["hbm"] if tk.get("bound") == "hbm" else pk["tf_sustained"],
                 "unit": tk.get("unit"), "frac": tk.get("frac"), "traffic": traffic, "traffic_note": traffic_note,
@@ -434,7 +459,7 @@ def run_product(args, cfg):
                                       + ("(all images of a detection batch share one vocabulary prompt, hipie_img.py:330-332: encoded once and broadcast)"
                                          if same_rows else "(one expression per image)"),
                        "e2e_scope": "HIPIE_IMG.forward (public API) incl. post-processing rows a20-a23, pinned-host images in, results out",
-                       "l2": "per-step working set (>= 1 GB activations per block) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (>= 1 GB activations per block) exceeds the 50 MB L2; no explicit flush",
                        "precision_mode": args.precision,
                        "launch": "eager" if graphed is None else "CUDA graph replay of the hot step (kernels captured once after warm-up)"},
             "clocks": clk.summary(),
@@ -456,12 +481,17 @@ def main():
                     help="bf16x3 = parity-grade split precision (default, the headline); bf16 = fast mode")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch the hot step eagerly instead of replaying a CUDA graph")
-    ap.add_argument("--ref-budget-s", type=float, default=240.0, help="wall-clock budget of the --impl reference run")
+    ap.add_argument("--ref-budget-s", type=float, default=240.0,
+                    help="wall-clock budget of the --impl reference run: it stops before --steps samples when the next one would exceed it")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, at most 64 MB in all)")
     args = ap.parse_args()
-    # stdout carries exactly one JSON line.  NCCL_DEBUG is left as the caller set it (the driver reads the NCCL log for its
-    # evidence); NCCL prints its log to stdout by default, so it is routed to stderr instead of being silenced.
+    # stdout carries exactly one JSON line.  NCCL_DEBUG is left as the caller set it; NCCL prints its log to stdout by default,
+    # so it is routed to stderr instead of being silenced.
     if int(os.environ.get("WORLD_SIZE", "1")) > 1 and os.environ.get("NCCL_DEBUG", ""):
         os.environ.setdefault("NCCL_DEBUG_FILE", "/dev/stderr")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes what the GPU path computed; the reference arm (--impl reference) has no such outputs")
     cfg = CONFIGS[args.config]
     if args.impl == "reference":
         run_reference(args, cfg)

@@ -1,4 +1,4 @@
-"""hipie_b200 — B200-native (sm_100a) implementation of HIPIE's inference hot path.
+"""hipie_b200 — H100-native (sm_90a) implementation of HIPIE's inference hot path.
 
 Host side mirrors the reference's detectron2 / HIPIE operator interfaces; all hot ops go through the
 C-ABI shared library `libhipie_b200.so` (include/hipie_b200.h).  There is no CPU fallback: calling an

@@ -75,9 +75,6 @@ SYMBOLS = {
     "hipie_attention_tc_planes": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int,
                                    c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_int64, c_int64, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
-    "hipie_attention_tc_traced": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int,
-                                          c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                                          c_int64, c_int64, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p]),
     "hipie_relpos_bias": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_int, c_int,
                                   c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "hipie_relpos_bias_tc": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int, c_int, c_int,
@@ -113,8 +110,6 @@ def load():
         fn.restype = res
         fn.argtypes = args
     _lib = lib
-    if os.environ.get("HIPIE_GEMM_CTA_PAIRS", "") in ("0", "1"):       # A/B switch (tools/gemm_check.py, bench)
-        lib.hipie_set_option(b"gemm_cta_pairs", int(os.environ["HIPIE_GEMM_CTA_PAIRS"]))
     return lib
 
 

@@ -1,4 +1,4 @@
-"""Build libhipie_b200.so in-tree with nvcc for sm_100a (no torch headers, pure C-ABI)."""
+"""Build libhipie_b200.so in-tree with nvcc for the H100 (sm_90a; no torch headers, pure C-ABI)."""
 import hashlib
 import os
 import subprocess
@@ -11,7 +11,7 @@ STAMP = os.path.join(HERE, ".libhipie_b200.stamp")
 
 SOURCES = ["core.cu", "msda.cu", "gemm_tc.cu", "norm.cu", "attention.cu", "attention_tc.cu", "misc.cu", "postproc.cu", "select.cu", "maskclip.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
     "-DHIPIE_BUILDING",
 ]

@@ -9,7 +9,6 @@
 // Round-1 implementation: warp-level mma.sync (m16n8k16 bf16, fp32 accumulate) with cp.async
 // double-buffered K/V tiles.  Operands are bf16 hi/lo planes; prec==3 evaluates
 // S = Qh.Kh + Qh.Kl + Ql.Kh and O += Ph.Vh + Ph.Vl + Pl.Vh so the result is fp32-class.
-// (The tcgen05/TMEM port of this kernel is the next step; see DESIGN.md.)
 #include "common.cuh"
 
 namespace hipie {

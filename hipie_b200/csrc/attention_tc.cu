@@ -1,34 +1,21 @@
-// tcgen05 flash attention for the ViT-H blocks (hd = 80), sm_100a: global 64-wide token grids (T % 256 == 0), 80-wide ones
+// wgmma flash attention for the ViT-H blocks (hd = 80), sm_90a (H100): global 64-wide token grids (T % 256 == 0), 80-wide ones
 // (1280-pixel inputs; T % 1280 == 0) and the 14x14 windows.
 //
-//   softmax((q*scale) k^T + rel_h[q, kh] + rel_w[q, kw]) v      (/root/reference/projects/HIPIE/hipie/backbone/vit.py:67-83,
-//                                                                 backbone/utils.py:96-125)
+//   softmax((q*scale) k^T + rel_h[q, kh] + rel_w[q, kw]) v      (reference hipie/backbone/vit.py:67-83, backbone/utils.py:96-125)
 //
-// One CTA = 256 query rows (two 128-row tiles) of one (batch, head); 384 threads in three warpgroups (setmaxnreg 216 / 216 / 72):
-//   warp 8      TMA producer: K tiles (64 keys x 80) and V^T tiles (80 x 64 keys) into a hardware-swizzled shared-memory
-//               ring (head dim 80 = one 128B-swizzled 64-wide box + one 32B-swizzled 16-wide box), plus the two Q lo tiles once
-//   warp 9 / 10 MMA issuers, one per query tile: S_t = Q_t K_j^T (M=128, N=64, K=80; A = Q hi in TENSOR MEMORY, TS mode) and
-//               O_t += P_t V_j (M=128, N=80, K=64; A = P in tensor memory).  QK_t(j+1) is issued as soon as the softmax warps
-//               hold S_t(j) in registers; the two issuers' streams interleave in the tensor pipe, so while one tile is in
-//               its softmax the pipe works for the other.  Latency-critical waits poll (mbarrier.test_wait)
-//   warps 0-3   softmax of tile 0, warps 4-7 softmax of tile 1: ONE THREAD PER QUERY ROW (no cross-warp max exchange):
-//               tcgen05.ld the 64 scores, scale + rel-pos bias, online softmax with lazy rescaling of the TMEM accumulator,
-//               P written back to TMEM with tcgen05.st as the A operand of the PV MMA
-//   global mode: rel_w hoisted in registers, one prefetched rel_h scalar per tile (a 64-key tile is one key row of the grid);
-//               80-wide grids keep the 64-key tiles: tile j starts at grid column (64 j) mod 80, which repeats every 5 tiles, so
-//               the loop is unrolled over the 5 phases and every rel_w index / row boundary is a compile-time constant
-//   window mode (T = 196, 14 x 14): one CTA per (window, head); keys padded to 4 x 64 and masked; the bias index
-//               (k / 14, k % 14) folds to constants in the unrolled 4-tile loop; V^T holds every window at a 200-column pitch
-//               because TMA box starts must be 16-byte aligned
-// Precision: PREC==3 evaluates Qh.Kh + Qh.Kl + Ql.Kh and Ph.Vh + Ph.Vl + Pl.Vh (bf16x3, fp32-class); PREC==1 plain bf16.
-// Tensor memory (512 columns): per tile S 64 | P hi/lo 64 | O 80 | Q hi 40; Q lo does not fit and is the one A operand
-// read from shared memory (5 of the 30 MMAs per key tile).
-// History (profiles/, DESIGN.md sec. 7): v1 kept Q and P in shared memory (3.1 ms per global block at B = 8); v2 moved both to
-// TMEM with one query tile per CTA and two softmax warps per row quarter (2.1 ms, ~45 % of the MMA peak, softmax-latency
-// bound); v3 two-tile ping-pong with one thread per row (1.56 ms); v5 (this) per-tile issuers + early QK + polled barriers
-// (1.48 ms, tensor pipe 62 % active, softmax warps issue-bound).
+// One CTA = 128 query rows of one (batch, head); 384 threads in three warpgroups:
+//   warpgroup 0     TMA producer (one thread): the Q tiles once, then K tiles (64 keys x 80) and V^T tiles (80 x 64 keys) into a
+//                   3-stage hardware-swizzled shared-memory ring (head dim 80 = one 128B-swizzled 64-wide box + one 32B-swizzled
+//                   16-wide box)
+//   warpgroups 1-2  64 query rows each: S = Q K^T (wgmma m64n64k16, both operands in shared memory), scale + rel-pos bias and the
+//                   online softmax on the register fragment, P packed in registers as the A operand of O += P V (wgmma m64n80k16,
+//                   A from registers), O in registers; the two warpgroups interleave on the tensor cores
+//   window mode (T = 196, 14 x 14): keys padded to 4 x 64 and masked; V^T holds every window at a 200-column pitch because TMA
+//                   box starts must be 16-byte aligned
+// Precision: PREC==3 evaluates Qh.Kh + Qh.Kl + Ql.Kh and Ph.Vh + Ph.Vl + Pl.Vh (bf16x3, fp32-class); PREC==1 plain bf16 (or fp16).
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace hipie {
 using namespace ptx;
@@ -36,40 +23,18 @@ using namespace ptx;
 int make_tmap_bf16(CUtensorMap* out, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int batch,
                    int64_t bstride, int box_rows, int box_cols);
 
-constexpr int FA_BM = 128, FA_BN = 64, FA_HD = 80, FA_STAGES = 3;
-// Three warpgroups: warps 0-3 softmax of query tile 0, warps 4-7 softmax of tile 1, warps 8-11 = TMA producer, MMA issuer of tile 0,
-// MMA issuer of tile 1, (idle).  The roles are warpgroup-aligned so that setmaxnreg can move registers from the three single-thread
-// roles (72 each) to the softmax threads (216 each: 64 scores + the hoisted rel_w row of up to 80 entries stay in registers;
-// at the launch-bound 168 the 64-wide variant spilled 15 registers and the 80-wide one 34).
-constexpr int FA_THREADS = 384;
-constexpr int FA_W_TMA = 8, FA_W_MMA0 = 9, FA_W_MMA1 = 10;
-constexpr int FA_REGS_SOFTMAX = 216, FA_REGS_ISSUE = 72;      // 256 * 216 + 128 * 72 = 384 * 168: no spills in any variant
-constexpr int FA_QT = 2;           // query tiles per CTA (ping-pong: one in softmax while the other is in the tensor pipe)
-// tensor-memory map (columns), per query tile t at column 256 * t
-constexpr int TM_TILE = 256;
-// Single-pass modes (PREC == 1: bf16 or fp16 operands) append a ROW OF ONES to every V^T tile, so the PV MMA (N = 96 instead of
-// 80) also accumulates the softmax denominator sum_k P[q, k] in output column 80: the 64 row-sum additions per tile leave the
-// exp phase, which is the serialised resource of the two softmax warps sharing a MUFU unit (see tile_body), and the denominator
-// is the sum of exactly the rounded probabilities the numerator used.  The 3-pass mode has no TMEM columns left for it.
-template <int PREC>
-struct FaTm {
-    static constexpr bool SUMCOL = PREC != 3;
-    static constexpr int S = 0;                        // 64 fp32 score columns
-    static constexpr int P = 64;                       // P hi: 32 columns of packed 16-bit pairs; (3-pass) P lo: next 32
-    static constexpr int Q = SUMCOL ? 96 : 208;        // Q hi: 40 columns of packed pairs (Q lo stays in shared memory)
-    static constexpr int O = SUMCOL ? 136 : 128;       // fp32 output columns: 80 (+ 16: column 80 = row sum, 81..95 zero)
-    static constexpr int ON = SUMCOL ? 96 : FA_HD;     // N of the PV MMA
-};
+constexpr int FA_BM = 64, FA_BN = 64, FA_HD = 80, FA_STAGES = 3;
+constexpr int FA_CONSUMERS = 2;                        // consumer warpgroups per CTA, FA_BM query rows each
+constexpr int FA_THREADS = 128 * (1 + FA_CONSUMERS);   // + the producer warpgroup (one TMA thread)
+constexpr int FA_OLD = FA_HD + 4;                      // row length (floats) of the staged output tile
 
 struct FaMaps {
     CUtensorMap k64[2], k16[2], vt[2];   // [hi, lo]
-    CUtensorMap q64, q16;                // Q lo plane (A operand of the Ql.Kh pass, shared memory)
+    CUtensorMap q64[2], q16[2];
 };
 
 struct FaParams {
-    const __nv_bfloat16 *q_hi, *q_lo;
-    int64_t q_bs, q_ts;
-    const float *rel_h, *rel_w;   // (B,H,T,kh), (B,H,T,64) or null
+    const float *rel_h, *rel_w;   // (B,H,T,kh), (B,H,T,kw) or null
     int kh;
     float* out_f32;
     __nv_bfloat16 *out_hi, *out_lo;
@@ -79,107 +44,95 @@ struct FaParams {
     int T_rows;          // rows per batch item of the output (o_bs / o_ts)
     int q_col0, k_col0;           // column of head 0 inside the q / k rows
     float scale_log2e;
-    long long* trace;             // debug: per-tile clock64 timestamps of CTA (0,0,0) or null
 };
 
 template <int PREC>
 struct FaSmem {
     static constexpr int NPL = PREC == 3 ? 2 : 1;
     static constexpr int K64 = FA_BN * 128, K16 = FA_BN * 32;
-    static constexpr int VT = FaTm<PREC>::ON * 128;   // (single-pass modes: + 16 rows, the first of them all ones)
-    static constexpr int V_TX = NPL * FA_HD * 128;    // bytes one stage receives by TMA
+    static constexpr int VT = FA_HD * 128;
     static constexpr int K_STAGE = NPL * (K64 + K16);
     static constexpr int V_STAGE = NPL * VT;
     static constexpr int Q64 = FA_BM * 128, Q16 = FA_BM * 32;
-    static constexpr int Q_TILE = PREC == 3 ? Q64 + Q16 : 0;
+    static constexpr int Q_TILE = NPL * (Q64 + Q16);
     static constexpr int OFF_V = FA_STAGES * K_STAGE;
     static constexpr int OFF_Q = OFF_V + FA_STAGES * V_STAGE;
-    static constexpr int OFF_BAR = OFF_Q + FA_QT * Q_TILE;
+    static constexpr int OFF_O = OFF_Q + FA_CONSUMERS * Q_TILE;
+    static constexpr int OFF_BAR = OFF_O + FA_CONSUMERS * FA_BM * FA_OLD * 4;
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
 
-template <int V> struct Phase { static constexpr int value = V; };
 constexpr int FA_GW2 = 80;        // second supported global grid width (1280-pixel inputs)
 constexpr int FA_WIN = 14, FA_WIN_T = FA_WIN * FA_WIN;     // window mode: 14 x 14 tokens, keys padded to 4 x 64
 constexpr int FA_WIN_TP = 200;   // window mode: column pitch of one window in V^T (TMA box starts must be 16-byte aligned)
 
+// S (+)= Q . K^T over the head dim 80: one 128B-swizzled 64-wide box (4 wgmmas) + one 32B-swizzled 16-wide box
+template <bool F16>
+__device__ __forceinline__ void fa_qk(float (&sacc)[32], uint32_t q, uint32_t k, int qoff16, int koff16, bool first) {
+    const uint64_t q64 = wg::desc<128>(q), q16 = wg::desc<32>(q + qoff16), k64 = wg::desc<128>(k), k16 = wg::desc<32>(k + koff16);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        if (F16) wg::ss_f16_n64(sacc, q64 + 2 * kk, k64 + 2 * kk, !(first && kk == 0));
+        else wg::ss_bf16_n64(sacc, q64 + 2 * kk, k64 + 2 * kk, !(first && kk == 0));
+    }
+    if (F16) wg::ss_f16_n64(sacc, q16, k16, 1);
+    else wg::ss_bf16_n64(sacc, q16, k16, 1);
+}
+
+template <bool F16>
+__device__ __forceinline__ void fa_pv(float (&o)[40], const uint32_t (&pa)[4][4], uint32_t v) {
+    const uint64_t dv = wg::desc<128>(v);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        if (F16) wg::rs_f16_n80(o, pa[kk], dv + 2 * kk, 1);
+        else wg::rs_bf16_n80(o, pa[kk], dv + 2 * kk, 1);
+    }
+}
+
 // F16 (with PREC == 1): q, k, v^T are IEEE fp16 planes and P is written as fp16: the single-pass QK^T / PV mode of the precision
-// map (DESIGN.md 3: 2^-12 operand rounding instead of bf16's 2^-9 keeps the 1e-3 mask-logit budget, measured in
-// profiles/r02_precision_emulation.txt and tests/test_fullsize_gpu.py).
-template <int PREC, bool WIN, bool F16, bool TRACE, int GW>
+// map (DESIGN.md 3: 2^-12 operand rounding instead of bf16's 2^-9).
+// GW: key-grid width of the rel-pos tables (64 or 80; FA_WIN in window mode).
+template <int PREC, bool WIN, bool F16, int GW>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
     using SM = FaSmem<PREC>;
-    using TM = FaTm<PREC>;
     constexpr int NPL = SM::NPL;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // stays in the shared address space (LDS / STS)
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
     uint64_t* k_full = bars;                       // [STAGES]
-    uint64_t* k_empty = k_full + FA_STAGES;
+    uint64_t* k_empty = k_full + FA_STAGES;        // [STAGES] one arrival per consumer warp
     uint64_t* v_full = k_empty + FA_STAGES;
     uint64_t* v_empty = v_full + FA_STAGES;
-    uint64_t* q_ready = v_empty + FA_STAGES;       // [2]  Q hi parked in TMEM (4 warps per tile)
-    uint64_t* qlo_full = q_ready + FA_QT;          // [2]  Q lo tile landed in shared memory (TMA)
-    uint64_t* s_full = qlo_full + FA_QT;           // [2]  QK(j) of tile t complete
-    uint64_t* s_empty = s_full + FA_QT;            // [2]  scores (j) of tile t are in registers (4 warps): QK(j+1) may overwrite S
-    uint64_t* p_full = s_empty + FA_QT;            // [2]  P(j) of tile t written (4 warps)
-    uint64_t* pv_done = p_full + FA_QT;            // [2]  PV(j) of tile t complete: P may be overwritten, O is current
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + FA_QT);
+    uint64_t* q_full = v_empty + FA_STAGES;        // [CONSUMERS]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q0 = blockIdx.x * (FA_QT * FA_BM), h = blockIdx.y, b = blockIdx.z;
+    const int q0 = blockIdx.x * (FA_CONSUMERS * FA_BM), h = blockIdx.y, b = blockIdx.z;
     const int ntiles = WIN ? (FA_WIN_T + FA_BN - 1) / FA_BN : p.T / FA_BN;     // window mode: 196 keys in 4 tiles, tail masked
-    const bool trace_cta = TRACE && p.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
 
-    if (warp == FA_W_TMA && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int i = 0; i < NPL; ++i) {
             prefetch_tmap(&maps.k64[i]); prefetch_tmap(&maps.k16[i]); prefetch_tmap(&maps.vt[i]);
+            prefetch_tmap(&maps.q64[i]); prefetch_tmap(&maps.q16[i]);
         }
-        if (PREC == 3) { prefetch_tmap(&maps.q64); prefetch_tmap(&maps.q16); }
-    }
-    if (warp == FA_W_MMA0) {
-        if (lane == 0) {
-            for (int i = 0; i < FA_STAGES; ++i) {
-                mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], FA_QT);      // released by both tiles' issuers
-                mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], FA_QT);
-            }
-            for (int i = 0; i < FA_QT; ++i) {
-                mbar_init(&q_ready[i], 4); mbar_init(&qlo_full[i], 1);
-                mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 4);
-                mbar_init(&p_full[i], 4); mbar_init(&pv_done[i], 1);
-            }
-            fence_barrier_init();
+        for (int i = 0; i < FA_STAGES; ++i) {
+            mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 4 * FA_CONSUMERS);
+            mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 4 * FA_CONSUMERS);
         }
-        __syncwarp();
-        tmem_alloc(tmem_ptr, 512);
-        tmem_relinquish();
+        for (int i = 0; i < FA_CONSUMERS; ++i) mbar_init(&q_full[i], 1);
+        fence_barrier_init();
     }
-    if (TM::SUMCOL) {
-        // rows 80..95 of every V^T stage: row 80 all ones (fp16 / bf16 1.0), the rest zero; TMA only ever rewrites rows 0..79
-        const uint32_t ones2 = F16 ? 0x3C003C00u : 0x3F803F80u;
-        for (int i = threadIdx.x; i < FA_STAGES * 512; i += FA_THREADS) {
-            const int st = i >> 9, w = i & 511;
-            reinterpret_cast<uint32_t*>(smem + SM::OFF_V + st * SM::V_STAGE + FA_HD * 128)[w] = w < 32 ? ones2 : 0u;
-        }
-        fence_proxy_async_smem();          // generic-proxy writes -> visible to the MMA's async-proxy reads
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp >= FA_W_TMA) {
-    setmaxnreg_dec<FA_REGS_ISSUE>();          // (register reallocation has to dominate the role's code: one branch per warpgroup)
-    if (warp == FA_W_TMA) {
+    if (warp < 4) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
-            if (PREC == 3) {
-                for (int t = 0; t < FA_QT; ++t) {
-                    uint8_t* qb = smem + SM::OFF_Q + t * SM::Q_TILE;
-                    mbar_arrive_expect_tx(&qlo_full[t], SM::Q_TILE);
-                    tma_load_3d(qb, &maps.q64, &qlo_full[t], p.q_col0 + h * FA_HD, q0 + t * FA_BM, b);
-                    tma_load_3d(qb + SM::Q64, &maps.q16, &qlo_full[t], p.q_col0 + h * FA_HD + 64, q0 + t * FA_BM, b);
+        if (threadIdx.x == 0) {
+            for (int c = 0; c < FA_CONSUMERS; ++c) {
+                uint8_t* qb = smem + SM::OFF_Q + c * SM::Q_TILE;
+                mbar_arrive_expect_tx(&q_full[c], SM::Q_TILE);
+                for (int pl = 0; pl < NPL; ++pl) {
+                    tma_load_3d(qb + pl * (SM::Q64 + SM::Q16), &maps.q64[pl], &q_full[c], p.q_col0 + h * FA_HD, q0 + c * FA_BM, b);
+                    tma_load_3d(qb + pl * (SM::Q64 + SM::Q16) + SM::Q64, &maps.q16[pl], &q_full[c], p.q_col0 + h * FA_HD + 64, q0 + c * FA_BM, b);
                 }
             }
             int s = 0;
@@ -193,340 +146,178 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
                     tma_load_3d(kb + pl * (SM::K64 + SM::K16) + SM::K64, &maps.k16[pl], &k_full[s], p.k_col0 + h * FA_HD + 64, j * FA_BN, b);
                 }
                 mbar_wait(&v_empty[s], ph ^ 1);
-                mbar_arrive_expect_tx(&v_full[s], SM::V_TX);
+                mbar_arrive_expect_tx(&v_full[s], SM::V_STAGE);
                 uint8_t* vb = smem + SM::OFF_V + s * SM::V_STAGE;
                 for (int pl = 0; pl < NPL; ++pl)
                     tma_load_3d(vb + pl * SM::VT, &maps.vt[pl], &v_full[s], b * (WIN ? FA_WIN_TP : p.T) + j * FA_BN, h * FA_HD, 0);
                 if (++s == FA_STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == FA_W_MMA0 || warp == FA_W_MMA1) {
-        // ===================== MMA issuers: one warp per query tile =====================
-        //   S_t = Q_t K_j^T  (A = Q hi in TMEM; the Ql.Kh pass takes Q lo from shared memory)     O_t += P_t V_j  (A = P in TMEM)
-        // QK_t(j+1) is issued as soon as the softmax warps have pulled S_t(j) into registers, so the next scores are ready
-        // before the current softmax finishes; PV_t(j) follows P_t(j).  The two issuers' instruction streams interleave in the
-        // tensor pipe (independent accumulators), which hides the dependent-accumulate latency of the small-N MMAs and keeps
-        // the pipe busy while one tile waits on its softmax.  Latency-critical waits poll (test_wait) instead of suspending.
-        const int t = warp - FA_W_MMA0;
-        constexpr uint32_t idesc_qk = F16 ? make_idesc_f16(FA_BM, FA_BN) : make_idesc_bf16(FA_BM, FA_BN);
-        constexpr uint32_t idesc_pv = F16 ? make_idesc_f16(FA_BM, TM::ON) : make_idesc_bf16(FA_BM, TM::ON);
-        const uint32_t tb = tmem_base + t * TM_TILE;
-        const uint32_t dS = tb + TM::S, dO = tb + TM::O, tq = tb + TM::Q, tp_hi = tb + TM::P, tp_lo = tb + TM::P + 32;
-        const uint32_t qb = smem_u32(smem + SM::OFF_Q + t * SM::Q_TILE);
-        auto issue_qk = [&](int j) {
-            const int st = j % FA_STAGES;
-            if (elect_one()) {
-                const uint32_t kb = smem_u32(smem + st * SM::K_STAGE);
-                const uint64_t k64h = make_kmajor_desc<128>(kb), k16h = make_kmajor_desc<32>(kb + SM::K64);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16_ts(dS, tq + 8 * k, k64h + 2 * k, idesc_qk, k > 0);
-                umma_f16_ts(dS, tq + 32, k16h, idesc_qk, 1);
-                if (PREC == 3) {
-                    const uint64_t k64l = make_kmajor_desc<128>(kb + SM::K64 + SM::K16), k16l = make_kmajor_desc<32>(kb + 2 * SM::K64 + SM::K16);
-                    const uint64_t q64l = make_kmajor_desc<128>(qb), q16l = make_kmajor_desc<32>(qb + SM::Q64);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(dS, tq + 8 * k, k64l + 2 * k, idesc_qk, 1);
-                    umma_f16_ts(dS, tq + 32, k16l, idesc_qk, 1);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16(dS, q64l + 2 * k, k64h + 2 * k, idesc_qk, 1);
-                    umma_f16(dS, q16l, k16h, idesc_qk, 1);
-                }
-                umma_commit(&s_full[t]);
-                umma_commit(&k_empty[st]);
-            }
-            __syncwarp();
-        };
-        auto issue_pv = [&](int j) {
-            const int st = j % FA_STAGES;
-            if (elect_one()) {
-                const uint32_t vb = smem_u32(smem + SM::OFF_V + st * SM::V_STAGE);
-                const uint64_t v_hi = make_kmajor_desc<128>(vb), v_lo = make_kmajor_desc<128>(vb + SM::VT);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16_ts(dO, tp_hi + 8 * k, v_hi + 2 * k, idesc_pv, (j | k) != 0);
-                if (PREC == 3) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(dO, tp_hi + 8 * k, v_lo + 2 * k, idesc_pv, 1);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(dO, tp_lo + 8 * k, v_hi + 2 * k, idesc_pv, 1);
-                }
-                umma_commit(&pv_done[t]);
-                umma_commit(&v_empty[st]);
-            }
-            __syncwarp();
-        };
-        mbar_wait(&k_full[0], 0);
-        mbar_wait(&q_ready[t], 0);
-        if (PREC == 3) mbar_wait(&qlo_full[t], 0);
-        tc_fence_after();
-        issue_qk(0);
-        for (int j = 0; j < ntiles; ++j) {
-            const bool trm = trace_cta && lane == 0 && j < 32;
-            if (j + 1 < ntiles) {
-                mbar_wait(&k_full[(j + 1) % FA_STAGES], ((j + 1) / FA_STAGES) & 1);
-                if (trm) p.trace[(j * 2 + t) * 8 + 4] = clock64();
-                mbar_wait_spin(&s_empty[t], j & 1);
-                tc_fence_after();
-                issue_qk(j + 1);
-            }
-            mbar_wait(&v_full[j % FA_STAGES], (j / FA_STAGES) & 1);
-            if (trm) p.trace[(j * 2 + t) * 8 + 5] = clock64();
-            mbar_wait_spin(&p_full[t], j & 1);
-            tc_fence_after();
-            if (trm) p.trace[(j * 2 + t) * 8 + 6] = clock64();
-            issue_pv(j);
-            if (trm) p.trace[(j * 2 + t) * 8 + 7] = clock64();
-        }
+        return;
     }
-    } else {
-        setmaxnreg_inc<FA_REGS_SOFTMAX>();
-        // ===================== softmax / epilogue: warps 0-3 own query tile 0, warps 4-7 tile 1; one thread per row ==========
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-        const int t = warp >> 2;                      // warps 0-3: tile 0, warps 4-7: tile 1
-        const int r = quarter * 32 + lane;            // row of the query tile == TMEM lane
-        const int qrow = q0 + t * FA_BM + r;
-        const uint32_t tm = tmem_base + ((uint32_t)(quarter * 32) << 16) + t * TM_TILE;
-        const bool has_rel = p.rel_h != nullptr;
-        constexpr float LOG2E = 1.4426950408889634f;
-        // ---- park this row of Q hi in TMEM (packed bf16 pairs = the TS-mode A operand layout) ----
-        {
-            const bool qok = !WIN || qrow < p.T;                      // window mode: rows 196..255 of the tile pair are padding
-            const int64_t qoff = (int64_t)b * p.q_bs + (int64_t)(qok ? qrow : 0) * p.q_ts + p.q_col0 + h * FA_HD;
-            const uint4* src = reinterpret_cast<const uint4*>(p.q_hi + qoff);
-            const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
+    // ===================== consumer warpgroup c: 64 query rows =====================
+    // wgmma fragment: this thread holds rows ra = 16 wq + lane / 4 and ra + 8, columns 8 j + 2 (lane % 4) + {0, 1}
+    const int c = (threadIdx.x >> 7) - 1, wq = warp & 3, tig = lane & 3;
+    const int ra = 16 * wq + (lane >> 2);
+    const int qrow[2] = {q0 + c * FA_BM + ra, q0 + c * FA_BM + ra + 8};
+    const bool has_rel = p.rel_h != nullptr;
+    const float* relw_row[2];
+    const float* relh_row[2];
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                uint32_t w[16];
-                const uint4 a0 = qok ? src[4 * c] : zero4, a1 = qok ? src[4 * c + 1] : zero4, a2 = qok ? src[4 * c + 2] : zero4,
-                            a3 = qok ? src[4 * c + 3] : zero4;
-                w[0] = a0.x; w[1] = a0.y; w[2] = a0.z; w[3] = a0.w; w[4] = a1.x; w[5] = a1.y; w[6] = a1.z; w[7] = a1.w;
-                w[8] = a2.x; w[9] = a2.y; w[10] = a2.z; w[11] = a2.w; w[12] = a3.x; w[13] = a3.y; w[14] = a3.z; w[15] = a3.w;
-                tmem_st_32x32b_x16(tm + TM::Q + 16 * c, w);
-            }
-            const uint4 a8 = qok ? src[8] : zero4, a9 = qok ? src[9] : zero4;
-            tmem_st_32x32b_x4(tm + TM::Q + 32, a8.x, a8.y, a8.z, a8.w);
-            tmem_st_32x32b_x4(tm + TM::Q + 36, a9.x, a9.y, a9.z, a9.w);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&q_ready[t]);
-        }
-        float rw[WIN ? FA_WIN : GW];          // rel_w row of this query (window mode: 14 entries, global: the grid width), log2 domain
-        float rhw[WIN ? FA_WIN : 1];          // window mode: the rel_h row as well (global mode streams one rel_h scalar per tile)
-        const float* relh_row = nullptr;
-        if (WIN) {
-            const bool qok = qrow < p.T;
-            const int64_t rowi = ((int64_t)b * p.H + h) * p.T + (qok ? qrow : 0);
-#pragma unroll
-            for (int i = 0; i < FA_WIN; ++i) {
-                rw[i] = has_rel ? __ldg(p.rel_w + rowi * FA_WIN + i) * LOG2E : 0.f;
-                rhw[i] = has_rel ? __ldg(p.rel_h + rowi * FA_WIN + i) * LOG2E : 0.f;
-            }
-        } else if (has_rel) {
-            const int64_t rowi = ((int64_t)b * p.H + h) * p.T + qrow;
-            const float* rwp = p.rel_w + rowi * GW;
-#pragma unroll
-            for (int i = 0; i < GW; i += 4) {
-                const float4 v = *reinterpret_cast<const float4*>(rwp + i);
-                rw[i] = v.x * LOG2E; rw[i + 1] = v.y * LOG2E; rw[i + 2] = v.z * LOG2E; rw[i + 3] = v.w * LOG2E;
-            }
-            relh_row = p.rel_h + rowi * p.kh;
-        }
-        float m = -INFINITY, l = 0.f;          // m: running reference max (log2 domain, incl. rel-pos terms)
-        if (t == 1) named_bar_arrive(1 + 2 * quarter, 64);      // exp-phase hand-off (see tile_body): tile 0 goes first
-        // raw rel_h table values of the next tile (scaled at use, so the prefetch stays in flight).  GW == 64: a 64-key tile is one
-        // key row of the grid.  GW == 80: a tile straddles at most two rows (a: the row of its first key, b: the next one)
-        float rh_next = (!WIN && has_rel) ? __ldg(relh_row) : 0.f;
-        float rh_next_b = (!WIN && GW != FA_BN && has_rel) ? __ldg(relh_row + 1) : 0.f;
-        // log2-domain score of key column i of tile j: global mode adds the hoisted rel_w entry (rel_h is per tile); window mode
-        // decomposes the key index into the 14 x 14 grid (indices fold to constants once the 4-tile loop is unrolled) and masks
-        // the 60 padding keys of the last tile
-        // (global mode, OFF = grid column of the tile's first key: (64 j) mod GW, a compile-time constant per tile phase)
-        auto score = [&](uint32_t sbits, const int j, const int i, const int OFF) -> float {
-            if (WIN) {
-                const int k = j * FA_BN + i;
-                if (k >= FA_WIN_T) return -INFINITY;
-                return fmaf(__uint_as_float(sbits), p.scale_log2e, rhw[k / FA_WIN]) + rw[k % FA_WIN];
-            }
-            return fmaf(__uint_as_float(sbits), p.scale_log2e, has_rel ? rw[WIN ? 0 : (OFF + i) % GW] : 0.f);
-        };
-        // PH: phase of the tile inside the period of lcm(64, GW) keys -- 0 for the 64-wide grid and the windows; 0..4 for the 80-wide
-        // grid, where tile j starts at grid column OFF = (64 PH) mod 80 and its keys [SPLIT, 64) belong to the next key row
-        auto tile_body = [&](const int j, auto ph_tag) {
-            constexpr int PH = decltype(ph_tag)::value;
-            constexpr int OFF = WIN ? 0 : (FA_BN * PH) % GW;
-            constexpr int SPLIT = (!WIN && OFF + FA_BN > GW) ? GW - OFF : FA_BN;
-            const bool tr = trace_cta && lane == 0 && (warp & 3) == 0 && j < 32;
-            const float rh = rh_next * LOG2E, rhb = rh_next_b * LOG2E;
-            if (!WIN && has_rel && j + 1 < ntiles) {                                     // prefetch for the next tile
-                const int r0n = GW == FA_BN ? j + 1 : (FA_BN * (j + 1)) / GW;
-                rh_next = __ldg(relh_row + r0n);
-                if (GW != FA_BN) rh_next_b = __ldg(relh_row + min(r0n + 1, p.kh - 1));
-            }
-            if (tr) p.trace[(j * 2 + t) * 8 + 0] = clock64();
-            mbar_wait_spin(&s_full[t], j & 1);
-            tc_fence_after();
-            if (tr) p.trace[(j * 2 + t) * 8 + 1] = clock64();
-            float tv[FA_BN];
-            {
-                uint32_t sv[32];
-                tmem_ld_32x32b_x32(tm + TM::S, sv);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) tv[i] = score(sv[i], j, i, OFF);
-                tmem_ld_32x32b_x32(tm + TM::S + 32, sv);
-                tmem_ld_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&s_empty[t]);      // scores are in registers: QK_t(j+1) may overwrite S_t
-#pragma unroll
-                for (int i = 0; i < 32; ++i) tv[32 + i] = score(sv[i], j, 32 + i, OFF);
-            }
-            // t_i = s_i*scale*log2e + rel_w_i ; rel_h is uniform over the tile -> folded into the max / exponent offset
-            float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, mxb[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-            for (int i = 0; i < FA_BN; ++i) {
-                if (i < SPLIT) mx[i & 3] = fmaxf(mx[i & 3], tv[i]);
-                else mxb[i & 3] = fmaxf(mxb[i & 3], tv[i]);
-            }
-            float tmax = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) + rh;
-            if (SPLIT < FA_BN) tmax = fmaxf(tmax, fmaxf(fmaxf(mxb[0], mxb[1]), fmaxf(mxb[2], mxb[3])) + rhb);
-            // lazy rescale: keep the running reference max unless the tile exceeds it by more than 2^8
-            const bool need = tmax > m + 8.f;
-            float corr = 1.f;
-            if (need) {
-                corr = ex2_approx(m - tmax);   // m == -inf -> 0
-                m = tmax;
-                l *= corr;
-            }
-            if (j > 0) {
-                mbar_wait(&pv_done[t], (j - 1) & 1);           // PV_t(j-1) retired: P_t is free and O_t is current (long done normally)
-                tc_fence_after();
-                if (__any_sync(0xffffffffu, need)) {           // warp-uniform: tcgen05.ld/st are warp-collective (rare once the max settles)
-                    for (int c = 0; c < TM::ON; c += 16) {       // (single-pass modes: incl. the row-sum column)
-                        uint32_t o[16];
-                        tmem_ld_32x32b_x16(tm + TM::O + c, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * corr);
-                        tmem_st_32x32b_x16(tm + TM::O + c, o);
-                    }
-                }
-            }
-            if (tr) p.trace[(j * 2 + t) * 8 + 2] = clock64();
-            // The two softmax warps of an SM sub-partition (tile 0: warp q, tile 1: warp 4+q) share one MUFU unit.  Left alone
-            // they run in lock step and their 64-ex2 phases collide (ncu r02: 16 cycles per MUFU.EX2, XU 43 % busy overall); a
-            // named-barrier hand-off makes the exp phases alternate, so one warp's exponentials overlap the other's TMEM loads,
-            // max reduction and mbarrier waits.
-            // exponent arguments now, outside the hand-off: the exp phase below is only ex2 + pack + tcgen05.st
-            {
-                const float off = m - rh, offb = m - rhb;
-#pragma unroll
-                for (int i = 0; i < FA_BN; ++i) tv[i] -= (i < SPLIT ? off : offb);
-            }
-            named_bar_sync(1 + 2 * quarter + t, 64);
-            float rs[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int c = 0; c < FA_BN; c += 16) {
-                uint32_t ph_[8], pl_[8];
-#pragma unroll
-                for (int i = 0; i < 16; i += 2) {
-                    const float e0 = ex2_approx(tv[c + i]), e1 = ex2_approx(tv[c + i + 1]);
-                    if (!TM::SUMCOL) rs[(i >> 1) & 3] += e0 + e1;
-                    if (PREC == 3) split2(e0, e1, ph_[i >> 1], pl_[i >> 1]);
-                    else ph_[i >> 1] = F16 ? pack_f16x2(e0, e1) : pack_bf16x2(e0, e1);
-                }
-                tmem_st_32x32b_x4(tm + TM::P + (c >> 1), ph_[0], ph_[1], ph_[2], ph_[3]);
-                tmem_st_32x32b_x4(tm + TM::P + (c >> 1) + 4, ph_[4], ph_[5], ph_[6], ph_[7]);
-                if (PREC == 3) {
-                    tmem_st_32x32b_x4(tm + TM::P + 32 + (c >> 1), pl_[0], pl_[1], pl_[2], pl_[3]);
-                    tmem_st_32x32b_x4(tm + TM::P + 32 + (c >> 1) + 4, pl_[4], pl_[5], pl_[6], pl_[7]);
-                }
-            }
-            if (t == 0 || j + 1 < ntiles) named_bar_arrive(1 + 2 * quarter + (t ^ 1), 64);   // the other tile's exp phase may start
-            if (!TM::SUMCOL) l += (rs[0] + rs[1]) + (rs[2] + rs[3]);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_full[t]);
-            if (tr) p.trace[(j * 2 + t) * 8 + 3] = clock64();
-        };
-        if (WIN) {
-#pragma unroll
-            for (int j = 0; j < (FA_WIN_T + FA_BN - 1) / FA_BN; ++j) tile_body(j, Phase<0>{});
-        } else if (GW == FA_BN) {
-            for (int j = 0; j < ntiles; ++j) tile_body(j, Phase<0>{});
-        } else {                           // 80-wide grid: 5 tiles = 4 key rows per period (the host checks T % 320 == 0)
-            for (int j = 0; j < ntiles; j += 5) {
-                tile_body(j, Phase<0>{}); tile_body(j + 1, Phase<1>{}); tile_body(j + 2, Phase<2>{});
-                tile_body(j + 3, Phase<3>{}); tile_body(j + 4, Phase<4>{});
-            }
-        }
-        // ---- epilogue: O / l ----
-        mbar_wait(&pv_done[t], (ntiles - 1) & 1);
-        tc_fence_after();
-        if (TM::SUMCOL) {                 // the denominator came out of the PV MMA: output column 80
-            uint32_t o[16];
-            tmem_ld_32x32b_x16(tm + TM::O + FA_HD, o);
-            tmem_ld_wait();
-            l = __uint_as_float(o[0]);
-        }
-        const float inv = 1.f / l;
-        const int64_t obase = (int64_t)b * p.o_bs + (int64_t)qrow * p.o_ts + (int64_t)h * FA_HD;
-        const bool row_ok = !WIN || qrow < p.T;
-        for (int c = 0; c < FA_HD; c += 16) {
-            uint32_t o[16];
-            tmem_ld_32x32b_x16(tm + TM::O + c, o);
-            tmem_ld_wait();
-            float f[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(o[i]) * inv;
-            if (row_ok && p.out_f32) {
-#pragma unroll
-                for (int i = 0; i < 16; i += 4)
-                    *reinterpret_cast<float4*>(p.out_f32 + obase + c + i) = make_float4(f[i], f[i + 1], f[i + 2], f[i + 3]);
-            }
-            if (row_ok && p.out_hi && p.out_e4m3) {
-                uint4 h0, h1, a8, b8;
-                uint2 t;
-                split4_f16_e4m3(make_float4(f[0], f[1], f[2], f[3]), t, a8.x, b8.x); h0.x = t.x; h0.y = t.y;
-                split4_f16_e4m3(make_float4(f[4], f[5], f[6], f[7]), t, a8.y, b8.y); h0.z = t.x; h0.w = t.y;
-                split4_f16_e4m3(make_float4(f[8], f[9], f[10], f[11]), t, a8.z, b8.z); h1.x = t.x; h1.y = t.y;
-                split4_f16_e4m3(make_float4(f[12], f[13], f[14], f[15]), t, a8.w, b8.w); h1.z = t.x; h1.w = t.y;
-                *reinterpret_cast<uint4*>(p.out_hi + obase + c) = h0;
-                *reinterpret_cast<uint4*>(p.out_hi + obase + c + 8) = h1;
-                uint8_t* o8 = reinterpret_cast<uint8_t*>(p.out_lo) + ((int64_t)b * p.T_rows + qrow) * 2 * p.o_ts + e4m3_slot0(h * FA_HD + c);
-                *reinterpret_cast<uint4*>(o8) = a8;              // slot 0 / slot 1 of 16 columns inside one 32-column group (common.cuh)
-                *reinterpret_cast<uint4*>(o8 + 32) = b8;
-            } else if (row_ok && p.out_hi) {
-                uint4 h0, h1, l0, l1;
-                split2(f[0], f[1], h0.x, l0.x); split2(f[2], f[3], h0.y, l0.y);
-                split2(f[4], f[5], h0.z, l0.z); split2(f[6], f[7], h0.w, l0.w);
-                split2(f[8], f[9], h1.x, l1.x); split2(f[10], f[11], h1.y, l1.y);
-                split2(f[12], f[13], h1.z, l1.z); split2(f[14], f[15], h1.w, l1.w);
-                *reinterpret_cast<uint4*>(p.out_hi + obase + c) = h0;
-                *reinterpret_cast<uint4*>(p.out_hi + obase + c + 8) = h1;
-                if (p.out_lo) {
-                    *reinterpret_cast<uint4*>(p.out_lo + obase + c) = l0;
-                    *reinterpret_cast<uint4*>(p.out_lo + obase + c + 8) = l1;
-                }
-            }
-            __syncwarp();          // window mode: padding rows skip the stores; reconverge before the next warp-collective tcgen05.ld
-        }
-        tc_fence_before();
+    for (int e = 0; e < 2; ++e) {
+        const int64_t rowi = ((int64_t)b * p.H + h) * p.T + (qrow[e] < p.T ? qrow[e] : 0);
+        relw_row[e] = has_rel ? p.rel_w + rowi * GW : nullptr;
+        relh_row[e] = has_rel ? p.rel_h + rowi * (WIN ? FA_WIN : p.kh) : nullptr;
     }
-    __syncthreads();
-    if (warp == FA_W_MMA0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    constexpr float LOG2E = 1.4426950408889634f;
+    const uint32_t qb = smem_u32(smem + SM::OFF_Q + c * SM::Q_TILE);
+    float o[40];
+#pragma unroll
+    for (int i = 0; i < 40; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};     // running max (log2 domain) / this thread's share of the row sum
+    mbar_wait(&q_full[c], 0);
+    for (int j = 0; j < ntiles; ++j) {
+        const int s = j % FA_STAGES;
+        const uint32_t par = (j / FA_STAGES) & 1;
+        // ---- S = Q K^T (PREC 3: Qh.Kh + Qh.Kl + Ql.Kh) ----
+        mbar_wait(&k_full[s], par);
+        float sacc[32];
+        const uint32_t kb = smem_u32(smem + s * SM::K_STAGE);
+        wg::fence();
+        fa_qk<F16>(sacc, qb, kb, SM::Q64, SM::K64, true);
+        if (PREC == 3) {
+            fa_qk<F16>(sacc, qb, kb + SM::K64 + SM::K16, SM::Q64, SM::K64, false);
+            fa_qk<F16>(sacc, qb + SM::Q64 + SM::Q16, kb, SM::Q64, SM::K64, false);
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs(sacc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&k_empty[s]);
+        // ---- scores in the log2 domain: s * scale * log2e + (rel_h[q, key row] + rel_w[q, key column]) * log2e ----
+        float tmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int e = (i >> 1) & 1;
+            const int k = j * FA_BN + 8 * (i >> 2) + 2 * tig + (i & 1);
+            float t = sacc[i] * p.scale_log2e;
+            if (WIN && k >= FA_WIN_T) t = -INFINITY;
+            else if (has_rel) t = fmaf(__ldg(relh_row[e] + k / GW) + __ldg(relw_row[e] + k % GW), LOG2E, t);
+            sacc[i] = t;
+            tmax[e] = fmaxf(tmax[e], t);
+        }
+        float corr[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            tmax[e] = fmaxf(tmax[e], __shfl_xor_sync(0xffffffffu, tmax[e], 1));
+            tmax[e] = fmaxf(tmax[e], __shfl_xor_sync(0xffffffffu, tmax[e], 2));
+            const float mn = fmaxf(m[e], tmax[e]);
+            corr[e] = ex2_approx(m[e] - mn);      // m == -inf -> 0
+            m[e] = mn;
+            l[e] *= corr[e];
+        }
+#pragma unroll
+        for (int i = 0; i < 40; ++i) o[i] *= corr[(i >> 1) & 1];
+        // ---- P = exp2(t - m) as the register A operand of the PV wgmma (fragment of S == fragment of A, 16 keys per k-step) ----
+        uint32_t pa_hi[4][4], pa_lo[4][4];
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+            const int e = (i >> 1) & 1;
+            const float e0 = ex2_approx(sacc[i] - m[e]), e1 = ex2_approx(sacc[i + 1] - m[e]);
+            uint32_t hi, lo = 0u;
+            if (PREC == 3) {
+                split2(e0, e1, hi, lo);
+                l[e] += e0 + e1;
+            } else if (F16) {
+                hi = pack_f16x2(e0, e1);                   // the denominator sums exactly the rounded probabilities the numerator uses
+                const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                l[e] += r.x + r.y;
+            } else {
+                hi = pack_bf16x2(e0, e1);
+                l[e] += __uint_as_float(hi << 16) + __uint_as_float(hi & 0xffff0000u);
+            }
+            pa_hi[i >> 3][(i >> 1) & 3] = hi;
+            pa_lo[i >> 3][(i >> 1) & 3] = lo;
+        }
+        // ---- O += P V (PREC 3: Ph.Vh + Ph.Vl + Pl.Vh) ----
+        mbar_wait(&v_full[s], par);
+        const uint32_t vb = smem_u32(smem + SM::OFF_V + s * SM::V_STAGE);
+        wg::fence_regs(o);
+        wg::fence();
+        fa_pv<F16>(o, pa_hi, vb);
+        if (PREC == 3) {
+            fa_pv<F16>(o, pa_hi, vb + SM::VT);
+            fa_pv<F16>(o, pa_lo, vb);
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&v_empty[s]);
+    }
+    // ---- epilogue: O / l, staged row-major so that one thread writes 16 consecutive columns of one row ----
+    float* os = reinterpret_cast<float*>(smem + SM::OFF_O) + c * FA_BM * FA_OLD;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+        l[e] += __shfl_xor_sync(0xffffffffu, l[e], 1);
+        l[e] += __shfl_xor_sync(0xffffffffu, l[e], 2);
+        const float inv = 1.f / l[e];
+#pragma unroll
+        for (int jj = 0; jj < 10; ++jj)
+            *reinterpret_cast<float2*>(os + (ra + 8 * e) * FA_OLD + 8 * jj + 2 * tig) = make_float2(o[4 * jj + 2 * e] * inv, o[4 * jj + 2 * e + 1] * inv);
+    }
+    named_bar_sync(1 + c, 128);
+    const int t128 = threadIdx.x & 127;
+    const int r = t128 & 63, orow = q0 + c * FA_BM + r;
+    if (WIN && orow >= p.T) return;                 // window mode: rows 196..255 are padding
+    const int64_t obase = (int64_t)b * p.o_bs + (int64_t)orow * p.o_ts + (int64_t)h * FA_HD;
+    for (int cc = (t128 >> 6) * 16; cc < FA_HD; cc += 32) {
+        float f[16];
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+            const float4 v = *reinterpret_cast<const float4*>(os + r * FA_OLD + cc + i);
+            f[i] = v.x; f[i + 1] = v.y; f[i + 2] = v.z; f[i + 3] = v.w;
+        }
+        if (p.out_f32) {
+#pragma unroll
+            for (int i = 0; i < 16; i += 4)
+                *reinterpret_cast<float4*>(p.out_f32 + obase + cc + i) = make_float4(f[i], f[i + 1], f[i + 2], f[i + 3]);
+        }
+        if (p.out_hi && p.out_e4m3) {
+            uint4 h0, h1, a8, b8;
+            uint2 t;
+            split4_f16_e4m3(make_float4(f[0], f[1], f[2], f[3]), t, a8.x, b8.x); h0.x = t.x; h0.y = t.y;
+            split4_f16_e4m3(make_float4(f[4], f[5], f[6], f[7]), t, a8.y, b8.y); h0.z = t.x; h0.w = t.y;
+            split4_f16_e4m3(make_float4(f[8], f[9], f[10], f[11]), t, a8.z, b8.z); h1.x = t.x; h1.y = t.y;
+            split4_f16_e4m3(make_float4(f[12], f[13], f[14], f[15]), t, a8.w, b8.w); h1.z = t.x; h1.w = t.y;
+            *reinterpret_cast<uint4*>(p.out_hi + obase + cc) = h0;
+            *reinterpret_cast<uint4*>(p.out_hi + obase + cc + 8) = h1;
+            uint8_t* o8 = reinterpret_cast<uint8_t*>(p.out_lo) + ((int64_t)b * p.T_rows + orow) * 2 * p.o_ts + e4m3_slot0(h * FA_HD + cc);
+            *reinterpret_cast<uint4*>(o8) = a8;              // slot 0 / slot 1 of 16 columns inside one 32-column group (common.cuh)
+            *reinterpret_cast<uint4*>(o8 + 32) = b8;
+        } else if (p.out_hi) {
+            uint4 h0, h1, l0, l1;
+            split2(f[0], f[1], h0.x, l0.x); split2(f[2], f[3], h0.y, l0.y);
+            split2(f[4], f[5], h0.z, l0.z); split2(f[6], f[7], h0.w, l0.w);
+            split2(f[8], f[9], h1.x, l1.x); split2(f[10], f[11], h1.y, l1.y);
+            split2(f[12], f[13], h1.z, l1.z); split2(f[14], f[15], h1.w, l1.w);
+            *reinterpret_cast<uint4*>(p.out_hi + obase + cc) = h0;
+            *reinterpret_cast<uint4*>(p.out_hi + obase + cc + 8) = h1;
+            if (p.out_lo) {
+                *reinterpret_cast<uint4*>(p.out_lo + obase + cc) = l0;
+                *reinterpret_cast<uint4*>(p.out_lo + obase + cc + 8) = l1;
+            }
+        }
     }
 }
 
-template <int PREC, bool WIN, bool F16, bool TRACE = false, int GW = FA_BN>
+template <int PREC, bool WIN, bool F16, int GW = FA_BN>
 static int launch_fa(const FaMaps& maps, const FaParams& p, cudaStream_t st) {
     using SM = FaSmem<PREC>;
-    HIPIE_ENSURE_SMEM((attn_tc_kernel<PREC, WIN, F16, TRACE, GW>), SM::TOTAL);
-    dim3 grid(WIN ? 1 : p.T / (FA_QT * FA_BM), p.H, p.B);
-    attn_tc_kernel<PREC, WIN, F16, TRACE, GW><<<grid, FA_THREADS, SM::TOTAL, st>>>(maps, p);
+    HIPIE_ENSURE_SMEM((attn_tc_kernel<PREC, WIN, F16, GW>), SM::TOTAL);
+    constexpr int rows = FA_CONSUMERS * FA_BM;
+    dim3 grid(((WIN ? FA_WIN_T : p.T) + rows - 1) / rows, p.H, p.B);
+    attn_tc_kernel<PREC, WIN, F16, GW><<<grid, FA_THREADS, SM::TOTAL, st>>>(maps, p);
     HIPIE_CHECK_LAUNCH();
     return HIPIE_OK;
 }
@@ -539,7 +330,7 @@ static int attention_tc_impl(const void* q_hi, const void* q_lo, int64_t q_bs, i
                              const void* k_hi, const void* k_lo, int64_t k_bs, int64_t k_ts, int k_col0, int k_width,
                              const void* vt_hi, const void* vt_lo, int64_t vt_ld, const float* rel_h, const float* rel_w,
                              int kh, int kw, float* out_f32, void* out_hi, void* out_lo, int64_t o_bs, int64_t o_ts, int B,
-                             int H, int T, int hd, float scale, int prec, long long* trace, void* stream, int out_format) {
+                             int H, int T, int hd, float scale, int prec, void* stream, int out_format) {
     HIPIE_CHECK_ARG(out_format == 0 || (out_format == 1 && out_hi && out_lo && o_ts % 16 == 0 && o_bs % o_ts == 0 && o_ts == (int64_t)H * hd),
                     "hipie_attention_tc: out_format 1 (fp16 + e4m3 planes) needs out_hi, out_lo and contiguous (B, rows, H*hd) outputs");
     HIPIE_CHECK_ARG(q_hi && k_hi && vt_hi, "hipie_attention_tc: q/k/vt hi planes required");
@@ -548,7 +339,7 @@ static int attention_tc_impl(const void* q_hi, const void* q_lo, int64_t q_bs, i
     if (f16) prec = 1;
     HIPIE_CHECK_ARG(hd == FA_HD, "hipie_attention_tc: head dim must be 80 (got %d)", hd);
     const bool win = T == FA_WIN_T && kh == FA_WIN && kw == FA_WIN;      // 14 x 14 windows: one CTA per (window, head)
-    HIPIE_CHECK_ARG(win || (T > 0 && T % (FA_QT * FA_BM) == 0),
+    HIPIE_CHECK_ARG(win || (T > 0 && T % 256 == 0),
                     "hipie_attention_tc: T (%d) must be a multiple of 256 (or 196 with a 14x14 rel-pos grid: window mode)", T);
     HIPIE_CHECK_ARG((rel_h == nullptr) == (rel_w == nullptr), "hipie_attention_tc: rel_h and rel_w go together");
     const bool wide = !win && rel_h && kw == FA_GW2;       // 80-wide grid: 64-key tiles in 5 phases per 4 key rows
@@ -567,32 +358,23 @@ static int attention_tc_impl(const void* q_hi, const void* q_lo, int64_t q_bs, i
         if ((rc = make_tmap_bf16(&maps.vt[pl], vp[pl], (int64_t)H * FA_HD, (int64_t)B * (win ? FA_WIN_TP : T), vt_ld, 1, 0, FA_HD, 64))) return rc;
     }
     if (prec == 1) { maps.k64[1] = maps.k64[0]; maps.k16[1] = maps.k16[0]; maps.vt[1] = maps.vt[0]; }
-    const void* qsrc = prec == 3 ? q_lo : q_hi;     // prec 1 never loads it; keep the maps valid
-    if ((rc = make_tmap_bf16(&maps.q64, qsrc, T, q_width, q_ts, B, q_bs, FA_BM, 64))) return rc;
-    if ((rc = make_tmap_bf16(&maps.q16, qsrc, T, q_width, q_ts, B, q_bs, FA_BM, 16))) return rc;
+    const void* qp[2] = {q_hi, q_lo};
+    for (int pl = 0; pl < (prec == 3 ? 2 : 1); ++pl) {
+        if ((rc = make_tmap_bf16(&maps.q64[pl], qp[pl], T, q_width, q_ts, B, q_bs, FA_BM, 64))) return rc;
+        if ((rc = make_tmap_bf16(&maps.q16[pl], qp[pl], T, q_width, q_ts, B, q_bs, FA_BM, 16))) return rc;
+    }
+    if (prec == 1) { maps.q64[1] = maps.q64[0]; maps.q16[1] = maps.q16[0]; }
     FaParams p;
-    p.q_hi = (const __nv_bfloat16*)q_hi; p.q_lo = (const __nv_bfloat16*)q_lo; p.q_bs = q_bs; p.q_ts = q_ts;
     p.rel_h = rel_h; p.rel_w = rel_w; p.kh = kh;
     p.out_f32 = out_f32; p.out_hi = (__nv_bfloat16*)out_hi; p.out_lo = (__nv_bfloat16*)out_lo;
     p.out_e4m3 = out_format == 1 ? 1 : 0;
     p.T_rows = (int)(o_bs / o_ts);
     p.o_bs = o_bs; p.o_ts = o_ts; p.B = B; p.H = H; p.T = T; p.q_col0 = q_col0; p.k_col0 = k_col0;
     p.scale_log2e = scale * 1.4426950408889634f;
-    p.trace = trace;
     cudaStream_t st = (cudaStream_t)stream;
-    if (trace && !win && !wide) return prec == 3 ? launch_fa<3, false, false, true>(maps, p, st) : (f16 ? launch_fa<1, false, true, true>(maps, p, st) : launch_fa<1, false, false, true>(maps, p, st));
-    if (wide) return prec == 3 ? launch_fa<3, false, false, false, FA_GW2>(maps, p, st) : (f16 ? launch_fa<1, false, true, false, FA_GW2>(maps, p, st) : launch_fa<1, false, false, false, FA_GW2>(maps, p, st));
-    if (win) return prec == 3 ? launch_fa<3, true, false>(maps, p, st) : (f16 ? launch_fa<1, true, true>(maps, p, st) : launch_fa<1, true, false>(maps, p, st));
+    if (wide) return prec == 3 ? launch_fa<3, false, false, FA_GW2>(maps, p, st) : (f16 ? launch_fa<1, false, true, FA_GW2>(maps, p, st) : launch_fa<1, false, false, FA_GW2>(maps, p, st));
+    if (win) return prec == 3 ? launch_fa<3, true, false, FA_WIN>(maps, p, st) : (f16 ? launch_fa<1, true, true, FA_WIN>(maps, p, st) : launch_fa<1, true, false, FA_WIN>(maps, p, st));
     return prec == 3 ? launch_fa<3, false, false>(maps, p, st) : (f16 ? launch_fa<1, false, true>(maps, p, st) : launch_fa<1, false, false>(maps, p, st));
-}
-
-extern "C" int hipie_attention_tc_traced(const void* q_hi, const void* q_lo, int64_t q_bs, int64_t q_ts, int q_col0, int q_width,
-                                         const void* k_hi, const void* k_lo, int64_t k_bs, int64_t k_ts, int k_col0, int k_width,
-                                         const void* vt_hi, const void* vt_lo, int64_t vt_ld, const float* rel_h, const float* rel_w,
-                                         int kh, int kw, float* out_f32, void* out_hi, void* out_lo, int64_t o_bs, int64_t o_ts, int B,
-                                         int H, int T, int hd, float scale, int prec, long long* trace, void* stream) {
-    return attention_tc_impl(q_hi, q_lo, q_bs, q_ts, q_col0, q_width, k_hi, k_lo, k_bs, k_ts, k_col0, k_width, vt_hi, vt_lo, vt_ld, rel_h,
-                             rel_w, kh, kw, out_f32, out_hi, out_lo, o_bs, o_ts, B, H, T, hd, scale, prec, trace, stream, 0);
 }
 
 // Same attention with the output written as the operand planes of a prec-6 hipie_gemm (the proj linear): out_f16 (B, T, H*hd) one
@@ -603,7 +385,7 @@ extern "C" int hipie_attention_tc_planes(const void* q_hi, const void* q_lo, int
                                          int kh, int kw, float* out_f32, void* out_f16, void* out_e4m3, int64_t o_bs, int64_t o_ts, int B,
                                          int H, int T, int hd, float scale, int prec, void* stream) {
     return attention_tc_impl(q_hi, q_lo, q_bs, q_ts, q_col0, q_width, k_hi, k_lo, k_bs, k_ts, k_col0, k_width, vt_hi, vt_lo, vt_ld, rel_h,
-                             rel_w, kh, kw, out_f32, out_f16, out_e4m3, o_bs, o_ts, B, H, T, hd, scale, prec, nullptr, stream, 1);
+                             rel_w, kh, kw, out_f32, out_f16, out_e4m3, o_bs, o_ts, B, H, T, hd, scale, prec, stream, 1);
 }
 
 // Window mode (T == 196, kh == kw == 14): vt holds every window at a 200-column pitch, (H*80, B*200), pad columns zero.
@@ -614,6 +396,6 @@ extern "C" int hipie_attention_tc(const void* q_hi, const void* q_lo, int64_t q_
                                   const void* vt_hi, const void* vt_lo, int64_t vt_ld, const float* rel_h, const float* rel_w,
                                   int kh, int kw, float* out_f32, void* out_hi, void* out_lo, int64_t o_bs, int64_t o_ts, int B,
                                   int H, int T, int hd, float scale, int prec, void* stream) {
-    return hipie_attention_tc_traced(q_hi, q_lo, q_bs, q_ts, q_col0, q_width, k_hi, k_lo, k_bs, k_ts, k_col0, k_width, vt_hi, vt_lo, vt_ld, rel_h,
-                                     rel_w, kh, kw, out_f32, out_hi, out_lo, o_bs, o_ts, B, H, T, hd, scale, prec, nullptr, stream);
+    return attention_tc_impl(q_hi, q_lo, q_bs, q_ts, q_col0, q_width, k_hi, k_lo, k_bs, k_ts, k_col0, k_width, vt_hi, vt_lo, vt_ld, rel_h,
+                             rel_w, kh, kw, out_f32, out_hi, out_lo, o_bs, o_ts, B, H, T, hd, scale, prec, stream, 0);
 }

@@ -1,4 +1,4 @@
-// Shared host/device helpers for the hipie_b200 kernels (sm_100a only).
+// Shared host/device helpers for the hipie_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -66,7 +66,7 @@ static inline int num_sms() {
     if (n[dev] == 0) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        n[dev] = v > 0 ? v : 148;
+        n[dev] = v > 0 ? v : 132;
     }
     return n[dev];
 }

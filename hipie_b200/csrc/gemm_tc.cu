@@ -1,24 +1,21 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:
+// Persistent, warp-specialised wgmma GEMM for sm_90a (H100):
 //   C[b] = epilogue( alpha * A[b] . W[b]^T )      A: (M,K) bf16 K-major,  W: (N,K) bf16 K-major
 //
-// This one kernel carries every dense contraction of the hot path: the ViT-H qkv / proj / fc1 /
-// fc2 linears (/root/reference/projects/HIPIE/hipie/backbone/vit.py:67-83,212-230), the DETR /
-// MaskDINO / BERT linears, convolutions lowered to GEMM, and the MaskDINO mask-embed contraction
-// einsum("bqc,bchw->bqhw") (.../maskdino/transformer_decoder/maskdino_decoder.py:520-529) with the
+// This one kernel carries every dense contraction of the hot path: the ViT-H qkv / proj / fc1 / fc2 linears (reference
+// hipie/backbone/vit.py:67-83,212-230), the DETR / MaskDINO / BERT linears, convolutions lowered to GEMM, and the MaskDINO
+// mask-embed contraction einsum("bqc,bchw->bqhw") (.../maskdino/transformer_decoder/maskdino_decoder.py:520-529) with the
 // sigmoid-threshold fused as a bit-packed output.
 //
-// Structure (one CTA per SM, 576 threads):
-//   warp 0      TMA producer: cp.async.bulk.tensor tiles of A / W into a 4-stage 128B/64B-swizzled
-//               shared-memory ring, completion on mbarriers (expect_tx)
-//   warp 1      MMA issuer: one elected thread issues tcgen05.mma (M=128, N=BN, K=16) into a
-//               double-buffered fp32 accumulator in tensor memory; tcgen05.commit releases the
-//               smem stage / publishes the accumulator
-//   warps 2-17  epilogue: tcgen05.ld the accumulator (32 lanes x 32 columns per warp), transpose
-//               through padded smem so global stores are row-contiguous, fused bias / activation /
-//               layer-scale / residual / fp32 + bf16-split + bit-packed outputs
+// Structure (one CTA per SM, 384 threads, 128 x BN tiles, BN = 64 or 128):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor tiles of A / W into a 3-4 stage 128B/64B-swizzled
+//                   shared-memory ring, completion on mbarriers (expect_tx)
+//   warpgroups 1-2  consumers, 64 tile rows each: wgmma (m64 x BN x 16, both operands from shared memory) into fp32 register
+//                   accumulators, one k-block in flight; then the accumulator is staged row-major in shared memory and each warp
+//                   runs the epilogue on 32 rows x BN/2 columns: fused bias / activation / layer-scale / residual, fp32 + bf16-split +
+//                   bit-packed outputs, row-major through TMA stores where possible
 //
 // Precision: operands are bf16 "split" planes.  prec==1 uses hi only; prec==3 computes
-// Ahi.Whi + Ahi.Wlo + Alo.Whi in the same fp32 TMEM accumulator (error ~2^-16 relative, i.e.
+// Ahi.Whi + Ahi.Wlo + Alo.Whi in the same fp32 accumulator (error ~2^-16 relative, i.e.
 // fp32-class results from the bf16 tensor pipe), loading 4 tiles per 3 MMAs per k-block.
 // prec==4 is the two-pass fp16 mode of the precision map (DESIGN.md 3): A is ONE IEEE fp16 plane (an activation that is
 // rounded to fp16 downstream anyway: the LayerNorm output feeding qkv), W is fp16 hi + lo, A.Whi + A.Wlo -- the weight is exact
@@ -33,6 +30,7 @@
 // instruction's scale-input-d immediate (D = A.B + D * 2^-14).  Two pass-equivalents instead of three, same operand bytes.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include <mutex>
 #include <unordered_map>
 #include <string.h>
@@ -41,8 +39,9 @@ namespace hipie {
 using namespace ptx;
 
 constexpr int GEMM_BM = 128;
-constexpr int GEMM_EPI_WARPS = 16;
-constexpr int GEMM_THREADS = 64 + 32 * GEMM_EPI_WARPS;  // TMA warp, MMA warp, 16 epilogue warps
+constexpr int GEMM_CONSUMERS = 2;                            // warpgroups, 64 accumulator rows each
+constexpr int GEMM_EPI_WARPS = 4 * GEMM_CONSUMERS;
+constexpr int GEMM_THREADS = 128 + 128 * GEMM_CONSUMERS;     // producer warpgroup (one TMA thread) + the consumer warpgroups
 constexpr int EPI_LD = 16;  // row length (floats) of the epilogue transpose buffer; 16-byte groups are XOR-swizzled by row
 constexpr int EPI_WARP_BYTES = 4096;   // per epilogue warp: one 32 x 32 fp32 TMA-store box (or a 32 x 32 bf16 hi box + lo box)
 
@@ -62,7 +61,7 @@ struct GemmParams {
     float alpha;
     int transposed;  // 1: C stored as [N, ldc] (column-major output), lanes = rows; 2 / 3: the vectorised fp16-plane variant (8 / 4 rows per store)
     int tiles_m, tiles_n;
-    int f16_ops;     // operands are IEEE fp16 planes (single pass): fp16 instruction descriptor
+    int f16_ops;     // operands are IEEE fp16 planes: fp16 wgmma instead of bf16
     int relu_post;   // ReLU after the residual add
     int c_fp16;      // c_hi is one IEEE fp16 plane instead of bf16 hi/lo
     int c_e4m3;      // ... plus the e4m3 planes [e4m3(h) | e4m3(2^10 (x - h))] of the result (M x 2N, TMA-store path, map tm_c_lo)
@@ -73,31 +72,36 @@ struct GemmParams {
     int t_row_group, t_row_pad;   // transposed epilogue: row r -> r + (r / group) * pad (0 = off)
 };
 
-// CTAS == 2: a CTA pair (cluster of 2, the two SMs of a TPC) computes one 256 x BN tile with cta_group::2 MMAs: each CTA stages
-// its own 128 A rows and HALF of the W tile (the hardware shares the halves between the pair), which takes the shared-memory
-// traffic per k-block from 120 KB (over the 128 B/clk port budget: tensor pipe 76 % in round 1) to 80 KB.
-template <int PREC, int BN, int CTAS>
+template <int PREC, int BN>
 struct GemmCfg {
     static constexpr bool P4 = PREC == 4;
     static constexpr bool P6 = PREC == 6;                    // fp16 hi.hi sweep + e4m3 sweep for the two cross terms (see the header comment)
-    // elements per k-block of the 16-bit operands; BK*2 bytes == swizzle span.  (prec 4 on CTA pairs: 64-element blocks in 3 stages
-    // measured 4 % faster than 32-element blocks in 6 stages, tools/gemm_p4_micro.py)
-    static constexpr int BK = (PREC == 3 || (PREC == 4 && CTAS == 1)) ? 32 : 64;
+    static constexpr int BK = (PREC == 3 || P4) ? 32 : 64;   // elements per k-block of the 16-bit operands; BK*2 bytes == swizzle span
     static constexpr int BK8 = 128;                          // elements (= bytes) per k-block of the e4m3 sweep
     static constexpr int SWZ = BK * 2;
     static constexpr int A_TILE = GEMM_BM * BK * 2;          // bytes
-    static constexpr int W_ROWS = BN / CTAS;                 // W rows staged by one CTA
-    static constexpr int W_TILE = W_ROWS * BK * 2;
+    static constexpr int W_TILE = BN * BK * 2;
     static constexpr int A_PLANES = PREC == 3 ? 2 : 1, W_PLANES = (PREC == 3 || P4) ? 2 : 1;     // prec 6: one plane per sweep, same tile bytes
     static constexpr int STAGE = A_PLANES * A_TILE + W_PLANES * W_TILE;     // layout: A_hi | W_hi | (A_lo) | W_lo
+    static constexpr int ACC_LD = BN + 4;                    // fp32 accumulator tile staged for the epilogue: padded rows, lane = row reads
+    static constexpr int ACC_BYTES = GEMM_BM * ACC_LD * 4;  //   are conflict-free
     static constexpr int EPI_BYTES = GEMM_EPI_WARPS * EPI_WARP_BYTES;
-    static constexpr int SMEM_BUDGET = 232448 - 1024 - 256 - EPI_BYTES;                  // 227 KB per CTA
-    static constexpr int MAX_STAGES = CTAS == 2 ? 6 : 4;
+    static constexpr int SMEM_BUDGET = 232448 - 1024 - 256 - EPI_BYTES - ACC_BYTES;      // 227 KB per CTA
+    static constexpr int MAX_STAGES = 4;
     static constexpr int STAGES = SMEM_BUDGET / STAGE < MAX_STAGES ? SMEM_BUDGET / STAGE : MAX_STAGES;
     static_assert(STAGES >= 3, "pipeline too shallow");
-    static constexpr int SMEM = STAGES * STAGE + EPI_BYTES + 256 + 1024;
-    static constexpr int TMEM_COLS = 2 * BN >= 512 ? 512 : (2 * BN >= 256 ? 256 : (2 * BN >= 128 ? 128 : 64));
+    static constexpr int SMEM = STAGES * STAGE + ACC_BYTES + EPI_BYTES + 256 + 1024;
 };
+
+// NV fp32 values of one accumulator row (lane = row of the staged tile)
+template <int NV>
+__device__ __forceinline__ void acc_ld(const float* row, uint32_t (&v)[NV]) {
+#pragma unroll
+    for (int i = 0; i < NV; i += 4) {
+        const uint4 q = *reinterpret_cast<const uint4*>(row + i);
+        v[i] = q.x; v[i + 1] = q.y; v[i + 2] = q.z; v[i + 3] = q.w;
+    }
+}
 
 __device__ __forceinline__ float act_apply(float v, int act) {
     if (act == HIPIE_ACT_RELU) return fmaxf(v, 0.f);
@@ -143,10 +147,10 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
 }
 
 // Interior-tile row epilogue: all 32 rows and all columns of the warp's slice are in range, rows are 16-byte aligned and
-// not remapped.  No per-element predicates, 32-bit offsets from one tile base, the next chunk's tcgen05.ld is in flight
+// not remapped.  No per-element predicates, 32-bit offsets from one tile base, the next chunk's accumulator load is in flight
 // while the current chunk is converted and stored.
 template <int ACT>
-__device__ __forceinline__ void epilogue_rows_fast(const GemmParams& p, uint32_t taddr, uint32_t es, int b, int m0, int n0,
+__device__ __forceinline__ void epilogue_rows_fast(const GemmParams& p, const float* arow, uint32_t es, int b, int m0, int n0,
                                                    int col_begin, int col_end, int lane) {
     const int rsub = lane >> 2, c4 = (lane & 3) * 4;
     const int64_t tile_c = (int64_t)b * p.c_bstride + (int64_t)m0 * p.ldc + n0 + c4;
@@ -161,14 +165,13 @@ __device__ __forceinline__ void epilogue_rows_fast(const GemmParams& p, uint32_t
     const uint32_t wr = es + lane * (EPI_LD * 4);
     const uint32_t wsw = (lane >> 1) & 3;
     uint32_t v[16];
-    tmem_ld_32x32b_x16(taddr + col_begin, v);
+    acc_ld(arow + col_begin, v);
 #pragma unroll 1
     for (int cb = col_begin; cb < col_end; cb += 16) {
-        tmem_ld_wait();
 #pragma unroll
         for (int j = 0; j < 4; ++j) sts128(wr + ((j ^ wsw) << 4), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
         __syncwarp();
-        if (cb + 16 < col_end) tmem_ld_32x32b_x16(taddr + cb + 16, v);      // lands while this chunk is processed
+        if (cb + 16 < col_end) acc_ld(arow + cb + 16, v);
         float4 bias = make_float4(0.f, 0.f, 0.f, 0.f), cs = make_float4(1.f, 1.f, 1.f, 1.f);
         if (bias_t) bias = *reinterpret_cast<const float4*>(bias_t + cb);
         if (cs_t) cs = *reinterpret_cast<const float4*>(cs_t + cb);
@@ -205,7 +208,7 @@ __device__ __forceinline__ void epilogue_rows_fast(const GemmParams& p, uint32_t
 // (one per lane) are transposed through padded smem; afterwards lanes 0-7 cover one row with float4s, so a
 // warp stores four fully coalesced 128-byte row segments per instruction.
 template <int ACT>
-__device__ __forceinline__ void epilogue_rows(const GemmParams& p, uint32_t taddr, float* my_epi, int b, int m0,
+__device__ __forceinline__ void epilogue_rows(const GemmParams& p, const float* arow, float* my_epi, int b, int m0,
                                               int n0, int col_begin, int col_end, int lane) {
     const float* res_b = p.residual ? p.residual + (int64_t)b * p.r_bstride : nullptr;
     float* cf_b = p.c_f32 ? p.c_f32 + (int64_t)b * p.c_bstride : nullptr;
@@ -215,7 +218,7 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, uint32_t tadd
     const bool vec_ok = ((p.ldc & 3) == 0) && (!res_b || (p.ldr & 3) == 0);
     const int rmax = min(32, p.M - m0);
     if (vec_ok && !p.row_map && rmax == 32 && n0 + col_end <= p.N && 32 * p.ldc < (1ll << 30) && ((n0 & 3) == 0)) {
-        epilogue_rows_fast<ACT>(p, taddr, smem_u32(my_epi), b, m0, n0, col_begin, col_end, lane);
+        epilogue_rows_fast<ACT>(p, arow, smem_u32(my_epi), b, m0, n0, col_begin, col_end, lane);
         return;
     }
 #pragma unroll 1
@@ -223,8 +226,7 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, uint32_t tadd
         const int nbase = n0 + cb;
         if (nbase >= p.N) break;  // warp-uniform
         uint32_t v[16];
-        tmem_ld_32x32b_x16(taddr + cb, v);
-        tmem_ld_wait();
+        acc_ld(arow + cb, v);
 #pragma unroll
         for (int j = 0; j < 16; j += 4)     // 16-byte group g of row r lives at group g ^ ((r >> 1) & 3): conflict-free both ways
             *reinterpret_cast<uint4*>(my_epi + lane * EPI_LD + (((j >> 2) ^ ((lane >> 1) & 3)) << 2)) =
@@ -320,7 +322,7 @@ __device__ __forceinline__ float4 load4_guard(const float* p, int col, int N, fl
 // (x > threshold) output falls out of the layout for free: a lane's 32 columns are one 32-bit word of its row.
 template <int ACT>
 __device__ __forceinline__ void epilogue_rows_tma(const GemmParams& p, const CUtensorMap* tm_f32, const CUtensorMap* tm_hi,
-                                                  const CUtensorMap* tm_lo, uint32_t taddr, uint32_t sbuf, int b, int m0, int n0,
+                                                  const CUtensorMap* tm_lo, const float* arow, uint32_t sbuf, int b, int m0, int n0,
                                                   int col_begin, int col_end, int lane) {
     if (m0 >= p.M) return;          // warp-uniform: this 32-row group lies below the matrix
     const float alpha = p.alpha;
@@ -331,8 +333,7 @@ __device__ __forceinline__ void epilogue_rows_tma(const GemmParams& p, const CUt
         const int nbase = n0 + cb;
         if (nbase >= p.N) break;  // warp-uniform
         uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cb, v);
-        tmem_ld_wait();
+        acc_ld(arow + cb, v);
 #pragma unroll 1
         for (int pass = 0; pass < npass; ++pass) {
             const bool planes = p.c_hi && (pass == npass - 1) && !(p.c_f32 && pass == 0);
@@ -418,7 +419,7 @@ __device__ __forceinline__ void epilogue_rows_tma(const GemmParams& p, const CUt
 // VEC = 8 (16-byte stores) for plain outputs, VEC = 4 (8-byte stores) when rows are re-spaced per window (t_row_group / t_row_pad
 // multiples of 4 keep every 4-row run contiguous and 8-byte aligned).  Requires M % VEC == 0 and ldc % VEC == 0 (host-checked).
 template <int VEC>
-__device__ __forceinline__ void epilogue_transposed_f16(const GemmParams& p, uint32_t taddr, uint32_t sbuf, int b, int m0, int n0,
+__device__ __forceinline__ void epilogue_transposed_f16(const GemmParams& p, const float* arow, uint32_t sbuf, int b, int m0, int n0,
                                                         int col_begin, int col_end, int lane) {
     __half* c_b = reinterpret_cast<__half*>(p.c_hi) + (int64_t)b * p.c_bstride;
     constexpr int SEGS = 32 / VEC;                  // row segments per column
@@ -428,8 +429,7 @@ __device__ __forceinline__ void epilogue_transposed_f16(const GemmParams& p, uin
         const int nbase = n0 + cb;
         if (nbase >= p.N) break;
         uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cb, v);
-        tmem_ld_wait();
+        acc_ld(arow + cb, v);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
             float x = __uint_as_float(v[j]) * p.alpha;
@@ -463,7 +463,7 @@ __device__ __forceinline__ void epilogue_transposed_f16(const GemmParams& p, uin
 
 // Transposed epilogue (C stored [col * ldc + row]): lanes hold 32 consecutive rows, so each register j is a
 // coalesced 128-byte store along M; optional bit-packed (x > threshold) output packed along M.
-__device__ __forceinline__ void epilogue_transposed(const GemmParams& p, uint32_t taddr, int b, int m0, int n0,
+__device__ __forceinline__ void epilogue_transposed(const GemmParams& p, const float* arow, int b, int m0, int n0,
                                                     int col_begin, int col_end, int lane) {
     const float* res_b = p.residual ? p.residual + (int64_t)b * p.r_bstride : nullptr;
     float* cf_b = p.c_f32 ? p.c_f32 + (int64_t)b * p.c_bstride : nullptr;
@@ -476,8 +476,7 @@ __device__ __forceinline__ void epilogue_transposed(const GemmParams& p, uint32_
         const int nbase = n0 + cb;
         if (nbase >= p.N) break;
         uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cb, v);
-        tmem_ld_wait();
+        acc_ld(arow + cb, v);
         uint32_t bitsword = 0;
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
@@ -517,105 +516,106 @@ __device__ __forceinline__ void epilogue_transposed(const GemmParams& p, uint32_
     }
 }
 
-template <int PREC, int BN, int CTAS>
+// issue the wgmmas of one k-block for this warpgroup's 64 rows (A rows offset inside the stage by `a_off` bytes)
+template <int PREC, int BN>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t st, uint32_t a_off, bool f8, bool f16_ops, bool first) {
+    using Cfg = GemmCfg<PREC, BN>;
+    if (f8) {
+        // e4m3 sweep: 128-byte rows, 32 bytes along K per wgmma
+        const uint64_t da = wg::desc<128>(st + a_off), dw = wg::desc<128>(st + Cfg::A_TILE);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (BN == 64) wg::ss_e4m3_n64(*reinterpret_cast<float(*)[32]>(&acc), da + 2 * k, dw + 2 * k, !(first && k == 0));
+            else wg::ss_e4m3_n128(*reinterpret_cast<float(*)[64]>(&acc), da + 2 * k, dw + 2 * k, !(first && k == 0));
+        }
+        return;
+    }
+    auto mma = [&](uint64_t da, uint64_t dw, int scale_d) {
+        if (f16_ops) {
+            if (BN == 64) wg::ss_f16_n64(*reinterpret_cast<float(*)[32]>(&acc), da, dw, scale_d);
+            else wg::ss_f16_n128(*reinterpret_cast<float(*)[64]>(&acc), da, dw, scale_d);
+        } else {
+            if (BN == 64) wg::ss_bf16_n64(*reinterpret_cast<float(*)[32]>(&acc), da, dw, scale_d);
+            else wg::ss_bf16_n128(*reinterpret_cast<float(*)[64]>(&acc), da, dw, scale_d);
+        }
+    };
+    const uint64_t a_hi = wg::desc<Cfg::SWZ>(st + a_off), w_hi = wg::desc<Cfg::SWZ>(st + Cfg::A_TILE);
+    // 16 elements (32 bytes) along K per wgmma inside the swizzle atom: +2 in addr>>4 units
+#pragma unroll
+    for (int k = 0; k < Cfg::BK / 16; ++k) mma(a_hi + 2 * k, w_hi + 2 * k, !(first && k == 0));
+    if (Cfg::P4) {
+        const uint64_t w_lo = wg::desc<Cfg::SWZ>(st + Cfg::A_TILE + Cfg::W_TILE);
+#pragma unroll
+        for (int k = 0; k < Cfg::BK / 16; ++k) mma(a_hi + 2 * k, w_lo + 2 * k, 1);
+    }
+    if (PREC == 3) {
+        const uint64_t a_lo = wg::desc<Cfg::SWZ>(st + Cfg::A_TILE + Cfg::W_TILE + a_off);
+        const uint64_t w_lo = wg::desc<Cfg::SWZ>(st + 2 * Cfg::A_TILE + Cfg::W_TILE);
+#pragma unroll
+        for (int k = 0; k < Cfg::BK / 16; ++k) mma(a_hi + 2 * k, w_lo + 2 * k, 1);
+#pragma unroll
+        for (int k = 0; k < Cfg::BK / 16; ++k) mma(a_lo + 2 * k, w_hi + 2 * k, 1);
+    }
+}
+
+template <int PREC, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
                const __grid_constant__ CUtensorMap tm_c_f32, const __grid_constant__ CUtensorMap tm_c_hi,
                const __grid_constant__ CUtensorMap tm_c_lo, const GemmParams p) {
-    using Cfg = GemmCfg<PREC, BN, CTAS>;
+    using Cfg = GemmCfg<PREC, BN>;
     constexpr int BK = Cfg::BK;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
-    // same CTA-relative offsets in both CTAs of a pair (the dynamic shared window starts at the same offset in every CTA of a
-    // launch), which the pair MMA descriptors and the multicast commits rely on
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // stays in the shared address space (LDS / STS)
     uint8_t* stage_base = smem;
-    float* epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE + Cfg::EPI_BYTES);
-    uint64_t* full_bar = bars;                // [STAGES]  (pair: only the leader's are used)
-    uint64_t* empty_bar = bars + STAGES;      // [STAGES]
-    uint64_t* tfull_bar = bars + 2 * STAGES;  // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;     // [2]       (pair: only the leader's are used)
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+    float* acc_s = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE);
+    float* epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE + Cfg::ACC_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE + Cfg::ACC_BYTES + Cfg::EPI_BYTES);
+    uint64_t* full_bar = bars;                // [STAGES]
+    uint64_t* empty_bar = bars + STAGES;      // [STAGES]  one arrival per consumer warp
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
-    const bool leader = rank == 0;
     const int num_kb8 = Cfg::P6 ? (2 * p.K + Cfg::BK8 - 1) / Cfg::BK8 : 0;     // k-blocks of the e4m3 sweep (planes are 2K wide)
     const int num_kb = num_kb8 + (p.K + BK - 1) / BK;
-    const int tiles_per_batch = p.tiles_m * p.tiles_n;      // tiles_m counts (128 * CTAS)-row tiles
+    const int tiles_per_batch = p.tiles_m * p.tiles_n;
     const int total_tiles = tiles_per_batch * p.batch;
-    const int tile0 = blockIdx.x / CTAS, tile_step = gridDim.x / CTAS;
 
-    if (CTAS == 2) cluster_sync();             // both CTAs of the pair are resident before the paired TMEM allocation
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&tm_a_hi);
         prefetch_tmap(&tm_w_hi);
-        if (PREC == 3) prefetch_tmap(&tm_a_lo);
-        if (PREC == 3 || Cfg::P4) prefetch_tmap(&tm_w_lo);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int i = 0; i < STAGES; ++i) {
-                mbar_init(&full_bar[i], 1);
-                mbar_init(&empty_bar[i], 1);
-            }
-            for (int i = 0; i < 2; ++i) {
-                mbar_init(&tfull_bar[i], 1);
-                mbar_init(&tempty_bar[i], GEMM_EPI_WARPS * CTAS);
-            }
-            fence_barrier_init();
+        if (PREC == 3 || Cfg::P6) prefetch_tmap(&tm_a_lo);
+        if (PREC == 3 || Cfg::P4 || Cfg::P6) prefetch_tmap(&tm_w_lo);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], GEMM_EPI_WARPS);
         }
-        __syncwarp();
-        if (CTAS == 2) {
-            tmem_alloc_2sm(tmem_ptr, Cfg::TMEM_COLS);
-            tmem_relinquish_2sm();
-        } else {
-            tmem_alloc(tmem_ptr, Cfg::TMEM_COLS);
-            tmem_relinquish();
-        }
+        fence_barrier_init();
     }
-    tc_fence_before();
-    if (CTAS == 2) cluster_sync(); else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
+    __syncthreads();
 
-    if (warp == 0) {
-        // ===================== TMA producer (one per CTA) =====================
-        if (lane == 0) {
+    if (warp < 4) {
+        // ===================== TMA producer (one thread) =====================
+        if (threadIdx.x == 0) {
             int s = 0;
             uint32_t ph = 0;
-            for (int t = tile0; t < total_tiles; t += tile_step) {
+            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
                 const int b = t / tiles_per_batch;
                 const int r = t - b * tiles_per_batch;
                 const int mt = p.m_fastest ? r % p.tiles_m : r / p.tiles_n, nt = p.m_fastest ? r / p.tiles_m : r - mt * p.tiles_n;
-                const int m0 = (mt * CTAS + (int)rank) * GEMM_BM, n0 = nt * BN + (int)rank * Cfg::W_ROWS;
+                const int m0 = mt * GEMM_BM, n0 = nt * BN;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(&empty_bar[s], ph ^ 1);
                     uint8_t* st = stage_base + s * Cfg::STAGE;
-                    if (Cfg::P6) {
+                    mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE);
+                    if (Cfg::P6 && kb < num_kb8) {
                         // sweep 1: e4m3 planes (maps tm_a_lo / tm_w_lo, 128-byte k-blocks); sweep 2: fp16 planes (64-element k-blocks)
-                        const bool f8 = kb < num_kb8;
-                        const int k0 = f8 ? kb * Cfg::BK8 : (kb - num_kb8) * BK;
-                        const CUtensorMap* ma = f8 ? &tm_a_lo : &tm_a_hi;
-                        const CUtensorMap* mw = f8 ? &tm_w_lo : &tm_w_hi;
-                        if (CTAS == 1) {
-                            mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE);
-                            tma_load_3d(st, ma, &full_bar[s], k0, m0, b);
-                            tma_load_3d(st + Cfg::A_TILE, mw, &full_bar[s], k0, n0, b);
-                        } else {
-                            if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::STAGE);
-                            tma_load_3d_2sm(st, ma, &full_bar[s], k0, m0, b);
-                            tma_load_3d_2sm(st + Cfg::A_TILE, mw, &full_bar[s], k0, n0, b);
-                        }
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                        continue;
-                    }
-                    const int k0 = kb * BK;
-                    if (CTAS == 1) {
-                        mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE);
+                        tma_load_3d(st, &tm_a_lo, &full_bar[s], kb * Cfg::BK8, m0, b);
+                        tma_load_3d(st + Cfg::A_TILE, &tm_w_lo, &full_bar[s], kb * Cfg::BK8, n0, b);
+                    } else {
+                        const int k0 = (kb - num_kb8) * BK;
                         tma_load_3d(st, &tm_a_hi, &full_bar[s], k0, m0, b);
                         tma_load_3d(st + Cfg::A_TILE, &tm_w_hi, &full_bar[s], k0, n0, b);
                         if (PREC == 3) {
@@ -623,174 +623,106 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
                             tma_load_3d(st + 2 * Cfg::A_TILE + Cfg::W_TILE, &tm_w_lo, &full_bar[s], k0, n0, b);
                         }
                         if (Cfg::P4) tma_load_3d(st + Cfg::A_TILE + Cfg::W_TILE, &tm_w_lo, &full_bar[s], k0, n0, b);
-                    } else {
-                        // both CTAs' loads report to the LEADER's barrier, which expects the bytes of the whole pair; the peer's
-                        // loads of this stage cannot run ahead of the phase (its empty barrier is released by the same commit)
-                        if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::STAGE);
-                        tma_load_3d_2sm(st, &tm_a_hi, &full_bar[s], k0, m0, b);
-                        tma_load_3d_2sm(st + Cfg::A_TILE, &tm_w_hi, &full_bar[s], k0, n0, b);
-                        if (PREC == 3) {
-                            tma_load_3d_2sm(st + Cfg::A_TILE + Cfg::W_TILE, &tm_a_lo, &full_bar[s], k0, m0, b);
-                            tma_load_3d_2sm(st + 2 * Cfg::A_TILE + Cfg::W_TILE, &tm_w_lo, &full_bar[s], k0, n0, b);
-                        }
-                        if (Cfg::P4) tma_load_3d_2sm(st + Cfg::A_TILE + Cfg::W_TILE, &tm_w_lo, &full_bar[s], k0, n0, b);
                     }
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (pair: the leader CTA only) =====================
-        if (leader) {
-            const uint32_t idesc = p.f16_ops ? make_idesc_f16(GEMM_BM * CTAS, BN) : make_idesc_bf16(GEMM_BM * CTAS, BN);
-            int s = 0;
-            uint32_t ph = 0;
-            int acc = 0;
-            uint32_t acc_ph = 0;
-            for (int t = tile0; t < total_tiles; t += tile_step) {
-                mbar_wait(&tempty_bar[acc], acc_ph ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t st = smem_u32(stage_base + s * Cfg::STAGE);
-                        const uint64_t a_hi = make_kmajor_desc<Cfg::SWZ>(st);
-                        const uint64_t w_hi = make_kmajor_desc<Cfg::SWZ>(st + Cfg::A_TILE);
-                        if (Cfg::P6) {
-                            // 32 bytes along K per MMA in both sweeps (32 e4m3 or 16 fp16 elements): +2 in addr>>4 units
-                            if (kb < num_kb8) {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) {
-                                    if (CTAS == 2) umma_f8_2sm(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, (kb | k) != 0);
-                                    else umma_f8(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, (kb | k) != 0);
-                                }
-                            } else {
-#pragma unroll
-                                for (int k = 0; k < 4; ++k) {
-                                    if (kb == num_kb8 && k == 0) {     // first fp16 MMA: D = A.B + D * 2^-14
-                                        if (CTAS == 2) umma_f16_2sm_scale14(d_tmem, a_hi, w_hi, idesc);
-                                        else umma_f16_scale14(d_tmem, a_hi, w_hi, idesc);
-                                    } else {
-                                        if (CTAS == 2) umma_f16_2sm(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, 1);
-                                        else umma_f16(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, 1);
-                                    }
-                                }
-                            }
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
-                                // advance 16 elements (32 bytes) along K inside the swizzle atom: +2 in addr>>4 units
-                                if (CTAS == 2) umma_f16_2sm(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, (kb | k) != 0);
-                                else umma_f16(d_tmem, a_hi + 2 * k, w_hi + 2 * k, idesc, (kb | k) != 0);
-                            }
-                        }
-                        if (Cfg::P4) {
-                            const uint64_t w_lo = make_kmajor_desc<Cfg::SWZ>(st + Cfg::A_TILE + Cfg::W_TILE);
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
-                                if (CTAS == 2) umma_f16_2sm(d_tmem, a_hi + 2 * k, w_lo + 2 * k, idesc, 1);
-                                else umma_f16(d_tmem, a_hi + 2 * k, w_lo + 2 * k, idesc, 1);
-                            }
-                        }
-                        if (PREC == 3) {
-                            const uint64_t a_lo = make_kmajor_desc<Cfg::SWZ>(st + Cfg::A_TILE + Cfg::W_TILE);
-                            const uint64_t w_lo = make_kmajor_desc<Cfg::SWZ>(st + 2 * Cfg::A_TILE + Cfg::W_TILE);
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
-                                if (CTAS == 2) umma_f16_2sm(d_tmem, a_hi + 2 * k, w_lo + 2 * k, idesc, 1);
-                                else umma_f16(d_tmem, a_hi + 2 * k, w_lo + 2 * k, idesc, 1);
-                            }
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
-                                if (CTAS == 2) umma_f16_2sm(d_tmem, a_lo + 2 * k, w_hi + 2 * k, idesc, 1);
-                                else umma_f16(d_tmem, a_lo + 2 * k, w_hi + 2 * k, idesc, 1);
-                            }
-                        }
-                        if (CTAS == 2) {
-                            umma_commit_2sm(&empty_bar[s], 3);                         // stage free in both CTAs
-                            if (kb == num_kb - 1) umma_commit_2sm(&tfull_bar[acc], 3);   // accumulator halves ready in both CTAs
-                        } else {
-                            umma_commit(&empty_bar[s]);                       // smem stage free when MMAs retire
-                            if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);  // accumulator ready
-                        }
-                    }
-                    __syncwarp();
-                    if (++s == STAGES) { s = 0; ph ^= 1; }
-                }
-                if (++acc == 2) { acc = 0; acc_ph ^= 1; }
             }
         }
     } else {
-        // ===================== epilogue (warps 2..17) =====================
-        // warp w may only touch TMEM lanes [32*(w%4), +32); four warps share a lane quarter and split
-        // the BN columns between them (the epilogue is latency-bound: more warps = more loads in flight).
-        const int quarter = warp & 3;
-        const int ew = warp - 2;                 // 0..15
-        const int cgroup = ew >> 2;              // which slice of the BN columns
-        float* my_epi = epi + ew * (EPI_WARP_BYTES / 4);          // 4 KB per warp (1024-byte aligned: TMA swizzle atoms)
+        // ===================== consumer warpgroups: wgmma mainloop + epilogue =====================
+        // warpgroup c owns rows [64 c, 64 c + 64) of the 128-row tile; the epilogue gives each of its warps 32 of those rows and half
+        // of the BN columns
+        const int c = (threadIdx.x >> 7) - 1;
+        const int wq = warp & 3;
+        const int ew = warp - 4;                              // 0..7
+        float* my_epi = epi + ew * (EPI_WARP_BYTES / 4);      // 4 KB per warp (1024-byte aligned: TMA swizzle atoms)
         const uint32_t my_sbuf = smem_u32(my_epi);
+        float* acc_tile = acc_s + c * 64 * Cfg::ACC_LD;
         if (p.tma_out && lane == 0) {
             if (p.c_f32) prefetch_tmap(&tm_c_f32);
             if (p.c_hi) prefetch_tmap(&tm_c_hi);
             if (p.c_lo || p.c_e4m3) prefetch_tmap(&tm_c_lo);
         }
-        constexpr int COLS_PER = BN / 4 >= 32 ? BN / 4 : 32;   // columns per warp (multiple of the 32-column transposed chunk)
-        const bool active = cgroup * COLS_PER < BN;
-        const int cbeg = cgroup * COLS_PER, cend = cbeg + COLS_PER;
-        int acc = 0;
-        uint32_t acc_ph = 0;
-        for (int t = tile0; t < total_tiles; t += tile_step) {
+        constexpr int COLS_PER = BN / 2;                      // columns per epilogue warp (a multiple of the 32-column chunk)
+        const int cbeg = (wq >> 1) * COLS_PER, cend = cbeg + COLS_PER;
+        const uint32_t a_off = (uint32_t)c * 64u * (uint32_t)Cfg::SWZ;            // 64 rows of the 16-bit A tile
+        const uint32_t a_off8 = (uint32_t)c * 64u * (uint32_t)Cfg::BK8;           // ... of the e4m3 A tile
+        int s = 0;
+        uint32_t ph = 0;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const int b = t / tiles_per_batch;
             const int r = t - b * tiles_per_batch;
             const int mt = p.m_fastest ? r % p.tiles_m : r / p.tiles_n, nt = p.m_fastest ? r / p.tiles_m : r - mt * p.tiles_n;
-            const int m0 = (mt * CTAS + (int)rank) * GEMM_BM + quarter * 32, n0 = nt * BN;
-            mbar_wait(&tfull_bar[acc], acc_ph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN;
-            if (active && m0 - quarter * 32 < p.M) {
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                const bool f8 = Cfg::P6 && kb < num_kb8;
+                if (Cfg::P6 && kb == num_kb8) {
+                    // the e4m3 sweep accumulated 2^14 x the cross terms: rescale before the fp16 sweep adds Ah.Wh
+                    wg::wait<0>();
+                    wg::fence_regs(acc);
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) acc[i] *= 0x1p-14f;
+                }
+                mbar_wait(&full_bar[s], ph);
+                wg::fence_regs(acc);
+                wg::fence();
+                gemm_kblock<PREC, BN>(acc, smem_u32(stage_base + s * Cfg::STAGE), f8 ? a_off8 : a_off, f8, p.f16_ops != 0, kb == 0);
+                wg::commit();
+                wg::wait<1>();                                   // the previous k-block's wgmmas have read their stage
+                wg::fence_regs(acc);
+                if (prev >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = s;
+                if (++s == STAGES) { s = 0; ph ^= 1; }
+            }
+            wg::wait<0>();
+            wg::fence_regs(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            // accumulator fragment -> staged tile (row-major, padded): d[4j + {0,1}] at (16 wq + lane / 4, 8 j + 2 (lane % 4)), +8 rows
+            {
+                const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    *reinterpret_cast<float2*>(acc_tile + r0 * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                    *reinterpret_cast<float2*>(acc_tile + (r0 + 8) * Cfg::ACC_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                }
+            }
+            named_bar_sync(1 + c, 128);
+            const int m0 = mt * GEMM_BM + c * 64 + (wq & 1) * 32, n0 = nt * BN;
+            const float* arow = acc_tile + ((wq & 1) * 32 + lane) * Cfg::ACC_LD;
+            if (m0 - (wq & 1) * 32 < p.M) {
                 if (p.transposed == 2)
-                    epilogue_transposed_f16<8>(p, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane);
+                    epilogue_transposed_f16<8>(p, arow, my_sbuf, b, m0, n0, cbeg, cend, lane);
                 else if (p.transposed == 3)
-                    epilogue_transposed_f16<4>(p, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane);
+                    epilogue_transposed_f16<4>(p, arow, my_sbuf, b, m0, n0, cbeg, cend, lane);
                 else if (p.transposed)
-                    epilogue_transposed(p, taddr, b, m0, n0, cbeg, cend, lane);
+                    epilogue_transposed(p, arow, b, m0, n0, cbeg, cend, lane);
                 else if (p.tma_out)
                     switch (p.act) {
-                        case HIPIE_ACT_RELU: epilogue_rows_tma<HIPIE_ACT_RELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
-                        case HIPIE_ACT_GELU: epilogue_rows_tma<HIPIE_ACT_GELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_RELU: epilogue_rows_tma<HIPIE_ACT_RELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, arow, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_GELU: epilogue_rows_tma<HIPIE_ACT_GELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, arow, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
                         case HIPIE_ACT_QUICK_GELU:
-                        case HIPIE_ACT_SIGMOID: epilogue_rows_tma<HIPIE_ACT_SIGMOID>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
-                        default: epilogue_rows_tma<HIPIE_ACT_NONE>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, taddr, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_SIGMOID: epilogue_rows_tma<HIPIE_ACT_SIGMOID>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, arow, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
+                        default: epilogue_rows_tma<HIPIE_ACT_NONE>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, arow, my_sbuf, b, m0, n0, cbeg, cend, lane); break;
                     }
                 else
                     switch (p.act) {
-                        case HIPIE_ACT_RELU: epilogue_rows<HIPIE_ACT_RELU>(p, taddr, my_epi, b, m0, n0, cbeg, cend, lane); break;
-                        case HIPIE_ACT_GELU: epilogue_rows<HIPIE_ACT_GELU>(p, taddr, my_epi, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_RELU: epilogue_rows<HIPIE_ACT_RELU>(p, arow, my_epi, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_GELU: epilogue_rows<HIPIE_ACT_GELU>(p, arow, my_epi, b, m0, n0, cbeg, cend, lane); break;
                         case HIPIE_ACT_QUICK_GELU:
-                        case HIPIE_ACT_SIGMOID: epilogue_rows<HIPIE_ACT_SIGMOID>(p, taddr, my_epi, b, m0, n0, cbeg, cend, lane); break;
-                        default: epilogue_rows<HIPIE_ACT_NONE>(p, taddr, my_epi, b, m0, n0, cbeg, cend, lane); break;
+                        case HIPIE_ACT_SIGMOID: epilogue_rows<HIPIE_ACT_SIGMOID>(p, arow, my_epi, b, m0, n0, cbeg, cend, lane); break;
+                        default: epilogue_rows<HIPIE_ACT_NONE>(p, arow, my_epi, b, m0, n0, cbeg, cend, lane); break;
                     }
             }
-            // all TMEM reads of this accumulator are complete -> hand it back to the MMA warp (of the leader CTA)
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (CTAS == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[acc]), 0));
-                else mbar_arrive(&tempty_bar[acc]);
-            }
-            if (++acc == 2) { acc = 0; acc_ph ^= 1; }
+            named_bar_sync(1 + c, 128);                       // the staged tile is read out before the next tile overwrites it
         }
         if (p.tma_out && lane == 0) bulk_wait0();     // outstanding TMA stores read this CTA's shared memory
-    }
-
-    tc_fence_before();
-    if (CTAS == 2) cluster_sync(); else __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        if (CTAS == 2) tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
-        else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
     }
 }
 
@@ -881,8 +813,7 @@ int make_tmap(CUtensorMap* out, const void* ptr, int esize, int64_t rows, int64_
     return HIPIE_OK;
 }
 
-// hipie_set_option switches (A/B measurements, fallbacks): CTA-pair (cta_group::2) tiles, TMA-store epilogue
-int g_gemm_cta_pairs = 1;
+// hipie_set_option switches (A/B measurements, fallbacks): TMA-store epilogue
 int g_gemm_tma_store = 1;
 int g_gemm_fast_transposed = 1;   // vectorised fp16-plane transposed epilogue (A/B switch)
 
@@ -910,22 +841,22 @@ int make_tmap_f32_5d(CUtensorMap* out, const void* ptr, const uint64_t dims[5], 
     return HIPIE_OK;
 }
 
-template <int PREC, int BN, int CTAS>
+template <int PREC, int BN>
 static int launch_gemm(const hipie_gemm_args* a, cudaStream_t st) {
-    using Cfg = GemmCfg<PREC, BN, CTAS>;
+    using Cfg = GemmCfg<PREC, BN>;
     CUtensorMap ta_hi, ta_lo, tw_hi, tw_lo;
     int rc;
     if ((rc = make_tmap_bf16(&ta_hi, a->a_hi, a->M, a->K, a->lda, a->batch, a->a_bstride, GEMM_BM, Cfg::BK))) return rc;
-    if ((rc = make_tmap_bf16(&tw_hi, a->w_hi, a->N, a->K, a->ldw, a->batch, a->w_bstride, Cfg::W_ROWS, Cfg::BK))) return rc;
+    if ((rc = make_tmap_bf16(&tw_hi, a->w_hi, a->N, a->K, a->ldw, a->batch, a->w_bstride, BN, Cfg::BK))) return rc;
     ta_lo = ta_hi;
     tw_lo = tw_hi;
     if (Cfg::P6) {       // e4m3 planes, 2K wide, 128-byte k-blocks
         if ((rc = make_tmap(&ta_lo, a->a8, 1, a->M, 2 * (int64_t)a->K, a->lda8, 1, 0, GEMM_BM, Cfg::BK8))) return rc;
-        if ((rc = make_tmap(&tw_lo, a->w8, 1, a->N, 2 * (int64_t)a->K, a->ldw8, 1, 0, Cfg::W_ROWS, Cfg::BK8))) return rc;
+        if ((rc = make_tmap(&tw_lo, a->w8, 1, a->N, 2 * (int64_t)a->K, a->ldw8, 1, 0, BN, Cfg::BK8))) return rc;
     }
     if (PREC == 3 && (rc = make_tmap_bf16(&ta_lo, a->a_lo, a->M, a->K, a->lda, a->batch, a->a_bstride, GEMM_BM, Cfg::BK))) return rc;
     if ((PREC == 3 || Cfg::P4) &&
-        (rc = make_tmap_bf16(&tw_lo, a->w_lo, a->N, a->K, a->ldw, a->batch, a->w_bstride, Cfg::W_ROWS, Cfg::BK))) return rc;
+        (rc = make_tmap_bf16(&tw_lo, a->w_lo, a->N, a->K, a->ldw, a->batch, a->w_bstride, BN, Cfg::BK))) return rc;
     // row-major outputs through TMA stores when nothing needs per-element addressing (residual / row map / transposed stay on the
     // register path) and the output rows satisfy TMA's 16-byte rules
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -967,28 +898,14 @@ static int launch_gemm(const hipie_gemm_args* a, cudaStream_t st) {
     p.row_map = a->c_row_map;
     p.t_row_group = a->transposed ? a->t_row_group : 0;
     p.t_row_pad = a->transposed ? a->t_row_pad : 0;
-    p.tiles_m = (a->M + GEMM_BM * CTAS - 1) / (GEMM_BM * CTAS);
+    p.tiles_m = (a->M + GEMM_BM - 1) / GEMM_BM;
     p.tiles_n = (a->N + BN - 1) / BN;
-    p.m_fastest = (p.tiles_m * CTAS <= 8 && p.tiles_n >= 4 * p.tiles_m * CTAS) ? 1 : 0;
+    p.m_fastest = (p.tiles_m <= 8 && p.tiles_n >= 4 * p.tiles_m) ? 1 : 0;
     const int64_t total = (int64_t)p.tiles_m * p.tiles_n * a->batch;
-    HIPIE_ENSURE_SMEM((gemm_tc_kernel<PREC, BN, CTAS>), Cfg::SMEM);
-    const int units = num_sms() / CTAS;      // CTAs (or CTA pairs) that can be resident
-    const int grid = (int)(total < units ? total : units) * CTAS;
-    if (CTAS == 1) {
-        gemm_tc_kernel<PREC, BN, CTAS><<<grid, GEMM_THREADS, Cfg::SMEM, st>>>(ta_hi, ta_lo, tw_hi, tw_lo, tc_f32, tc_hi, tc_lo, p);
-    } else {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(GEMM_THREADS);
-        cfg.dynamicSmemBytes = Cfg::SMEM;
-        cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = 1;
-        HIPIE_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<PREC, BN, CTAS>, ta_hi, ta_lo, tw_hi, tw_lo, tc_f32, tc_hi, tc_lo, p));
-    }
+    HIPIE_ENSURE_SMEM((gemm_tc_kernel<PREC, BN>), Cfg::SMEM);
+    const int units = num_sms();      // persistent: one CTA per SM
+    const int grid = (int)(total < units ? total : units);
+    gemm_tc_kernel<PREC, BN><<<grid, GEMM_THREADS, Cfg::SMEM, st>>>(ta_hi, ta_lo, tw_hi, tw_lo, tc_f32, tc_hi, tc_lo, p);
     HIPIE_CHECK_LAUNCH();
     return HIPIE_OK;
 }
@@ -1020,32 +937,19 @@ extern "C" int hipie_gemm(const hipie_gemm_args* a, void* stream) {
     HIPIE_CHECK_ARG(!a->c_fp16 || (a->c_hi && !a->c_lo), "hipie_gemm: c_fp16 writes one fp16 plane (c_hi set, c_lo NULL)");
     HIPIE_CHECK_ARG(!a->c_row_map || !a->transposed, "hipie_gemm: c_row_map is not supported with transposed=1");
     cudaStream_t st = (cudaStream_t)stream;
-    // CTA pairs where the mainloop dominates: big row counts, K >= 512, 3-pass operands (ViT / BERT / VL linears).  Measured on
-    // B200 (tools/gemm_check.py, profiles/r02_gemm_pairs.txt): fc1 32768x5120x1280 0.944 -> 0.844 ms, qk 0.489 -> 0.454 ms;
-    // K = 256 problems are epilogue/store-bound and lose 8-10 % with pairs, single-pass operands gain nothing.
-    const bool pairs = g_gemm_cta_pairs && a->M >= 1024 && a->N > 64 && a->K >= 512 && (a->prec == 3 || a->prec == 4 || a->prec == 6);
-    if (a->prec == 6) {                    // fp16 + e4m3 split (the large ViT linears)
-        if (a->N <= 128) return pairs ? launch_gemm<6, 128, 2>(a, st) : launch_gemm<6, 128, 1>(a, st);
-        return pairs ? launch_gemm<6, 256, 2>(a, st) : launch_gemm<6, 256, 1>(a, st);
-    }
-    if (a->prec == 4) {                    // two-pass fp16 (the qkv linears): wide outputs only
-        if (a->N <= 128) return pairs ? launch_gemm<4, 128, 2>(a, st) : launch_gemm<4, 128, 1>(a, st);
-        return pairs ? launch_gemm<4, 256, 2>(a, st) : launch_gemm<4, 256, 1>(a, st);
-    }
-    const bool p3 = a->prec == 3;          // prec 1 (bf16) and prec 2 (fp16) share the single-plane kernels; the MMA kind differs
-    if (a->N <= 64) return p3 ? launch_gemm<3, 64, 1>(a, st) : launch_gemm<1, 64, 1>(a, st);
-    if (a->N <= 128) {
-        if (pairs) return p3 ? launch_gemm<3, 128, 2>(a, st) : launch_gemm<1, 128, 2>(a, st);
-        return p3 ? launch_gemm<3, 128, 1>(a, st) : launch_gemm<1, 128, 1>(a, st);
-    }
-    if (pairs) return p3 ? launch_gemm<3, 256, 2>(a, st) : launch_gemm<1, 256, 2>(a, st);
-    return p3 ? launch_gemm<3, 256, 1>(a, st) : launch_gemm<1, 256, 1>(a, st);
+    // 128 x 64 tiles for narrow outputs, 128 x 128 otherwise (the fp32 accumulator of a 64-row warpgroup is 64 registers per
+    // thread at N = 128; its staged copy for the epilogue is what bounds the tile width in shared memory)
+    const bool narrow = a->N <= 64;
+    if (a->prec == 6) return narrow ? launch_gemm<6, 64>(a, st) : launch_gemm<6, 128>(a, st);   // fp16 + e4m3 split (the large ViT linears)
+    if (a->prec == 4) return narrow ? launch_gemm<4, 64>(a, st) : launch_gemm<4, 128>(a, st);   // two-pass fp16 (the qkv linears)
+    // prec 1 (bf16) and prec 2 (fp16) share the single-plane kernels; the wgmma type differs
+    if (a->prec == 3) return narrow ? launch_gemm<3, 64>(a, st) : launch_gemm<3, 128>(a, st);
+    return narrow ? launch_gemm<1, 64>(a, st) : launch_gemm<1, 128>(a, st);
 }
 
 extern int g_ln_grid_cap, g_ln_bulk;          // norm.cu (global scope)
 extern "C" int hipie_set_option(const char* name, int value) {
     HIPIE_CHECK_ARG(name != nullptr, "hipie_set_option: null name");
-    if (strcmp(name, "gemm_cta_pairs") == 0) { g_gemm_cta_pairs = value ? 1 : 0; return HIPIE_OK; }
     if (strcmp(name, "gemm_tma_store") == 0) { g_gemm_tma_store = value ? 1 : 0; return HIPIE_OK; }
     if (strcmp(name, "gemm_fast_transposed") == 0) { g_gemm_fast_transposed = value ? 1 : 0; return HIPIE_OK; }
     if (strcmp(name, "ln_grid_cap") == 0) { g_ln_grid_cap = value ? 1 : 0; return HIPIE_OK; }

@@ -1,4 +1,4 @@
-// Multi-scale deformable attention forward for sm_100a.
+// Multi-scale deformable attention forward for sm_90a.
 //
 // Semantics follow the reference operator `ms_deform_attn_forward`
 // (/root/reference/projects/HIPIE/hipie/models/deformable_detr/ops/src/cuda/ms_deform_attn_cuda.cu:20-78,

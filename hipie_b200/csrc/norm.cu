@@ -1,5 +1,5 @@
 // LayerNorm / GroupNorm for the hot path (fp32 statistics, fp32 and/or bf16-split outputs so the
-// normalised activations feed the tcgen05 GEMM without a separate conversion pass).
+// normalised activations feed the wgmma GEMM without a separate conversion pass).
 // Reference call sites: ViT pre-LN eps 1e-6 (/root/reference/projects/HIPIE/hipie/backbone/vit.py:212-230),
 // DETR / MaskDINO post-LN eps 1e-5 (deformable_transformer_dino.py:385-450), GroupNorm(32) of the
 // input projections (deformable_detr.py:221-236, maskdino_encoder.py:253-306).

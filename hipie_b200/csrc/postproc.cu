@@ -273,322 +273,10 @@ seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// tcgen05 version (C <= 80): the semantic contraction moves to the 5th-gen tensor cores; the CUDA cores only produce
-// sigmoid(bilinear()) and the panoptic bookkeeping.
-//   CTA = 32 x 8 pixels (two M=128 tiles: rows {0,1,4,5} and rows {2,3,6,7} of the patch, shifted by (-2,-2) so that every
-//   4x4 block shares its taps), 320 threads:
-//   warps 0-7   per 64-query chunk: thread = (pixel column, row pair); warps w and w+4 split the chunk's queries.  The thread
-//               evaluates both of its pixels (same 4 taps), keeps the panoptic argmax / area counts, and writes the sigmoid
-//               values as bf16 hi/lo pairs into TENSOR MEMORY (the A operand, like P in the attention kernel)
-//   warp 8      MMA issuer: D_t (128 px x 80 classes, fp32, TMEM) += A_t (TMEM) . P^T chunk (shared memory, K-major, 128B
-//               swizzle written by cp.async), bf16x3
-//   the chunk's class-probability tile is triple buffered, A double buffered; mbarriers throughout.
-// ------------------------------------------------------------------------------------------------------------------
 }  // namespace
 }  // namespace hipie
-#include "ptx.cuh"
 namespace hipie {
 namespace {
-using namespace ptx;
-
-constexpr int PT_CW = 16;                      // sigmoid / panoptic warps (4 per TMEM lane quarter, 16 queries of a chunk each)
-constexpr int PT_CT = PT_CW * 32;
-constexpr int PT_THREADS = PT_CT + 64;         // + MMA issuer warp (+1 idle warp keeps the count a multiple of 4 warps)
-constexpr int PT_NB = 3;                       // class-probability stages
-constexpr int PT_BTILE = 80 * 128;             // one plane of a P^T chunk: 80 classes x 64 queries bf16, 128-byte rows
-constexpr int PT_TM_D = 0;                     // D_A: 0..79, D_B: 80..159
-constexpr int PT_TM_A = 160;                   // + stage*128 + tile*64 (+32 for lo)
-
-struct PtSmem {
-    static constexpr int OFF_B = 0;                                  // [NB][hi,lo] swizzled tiles (1024-byte aligned)
-    static constexpr int OFF_TAPS = PT_NB * 2 * PT_BTILE;            // [2][64][27] floats
-    static constexpr int OFF_SC = OFF_TAPS + 2 * PP_QC * PP_TQ * 4;  // [2][64] floats
-    static constexpr int OFF_BAR = OFF_SC + 2 * PP_QC * 4;           // mbarriers + tmem ptr + exchange
-    static constexpr int OFF_X = OFF_BAR + 128;                      // argmax exchange: [3 other warps][256 px][value, index]
-    static constexpr int OFF_CNT = OFF_X + 3 * 256 * 2 * 4;
-};
-
-__global__ void __launch_bounds__(PT_THREADS, 1)
-seg_post_tc_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict__ pt_hi,
-                   const __nv_bfloat16* __restrict__ pt_lo, const float* __restrict__ scores, float* __restrict__ sem,
-                   int* __restrict__ ids, int* __restrict__ areas, int Q, int Qpad, int C, int h, int w, int Hc, int Wc) {
-    extern __shared__ uint8_t pt_raw[];
-    uint8_t* smem = pt_raw + ((1024u - (smem_u32(pt_raw) & 1023u)) & 1023u);   // stays in the shared address space (LDS / STS)
-    float* taps = reinterpret_cast<float*>(smem + PtSmem::OFF_TAPS);
-    float* sc = reinterpret_cast<float*>(smem + PtSmem::OFF_SC);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PtSmem::OFF_BAR);
-    uint64_t* a_full = bars;            // [2] 8 warps
-    uint64_t* a_empty = bars + 2;       // [2] umma commit
-    uint64_t* b_full = bars + 4;        // [NB] 1 arrive
-    uint64_t* b_empty = bars + 7;       // [NB] umma commit
-    uint64_t* d_full = bars + 10;       // [1]
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 11);
-    int* s_first = reinterpret_cast<int*>(bars + 12);
-    float* xch = reinterpret_cast<float*>(smem + PtSmem::OFF_X);
-    int* cnt = reinterpret_cast<int*>(smem + PtSmem::OFF_CNT);       // [3][Qpad]
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int kx0 = blockIdx.x * PP_BX, ky0 = blockIdx.y * PP_BY;
-    const int x_lo = kx0 - 1, y_lo = ky0 - 1;
-    const int nchunk = Qpad / PP_QC;
-
-    if (tid == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], PT_CW); mbar_init(&a_empty[i], 1); }
-        for (int i = 0; i < PT_NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-        mbar_init(d_full, 1);
-        *s_first = 0x7fffffff;
-        fence_barrier_init();
-    }
-    if (warp == PT_CW) {
-        tmem_alloc(tmem_ptr, 512);
-        tmem_relinquish();
-    }
-    for (int i = tid; i < 3 * Qpad; i += PT_THREADS) cnt[i] = 0;
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    for (int i = tid; i < Q; i += PT_THREADS)
-        if (scores[i] > 0.f) atomicMin(s_first, i);
-
-    if (warp == PT_CW) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = make_idesc_bf16(128, 80);
-        for (int ch = 0; ch < nchunk; ++ch) {
-            const int sa = ch & 1, sb = ch % PT_NB;
-            mbar_wait(&b_full[sb], (ch / PT_NB) & 1);
-            mbar_wait(&a_full[sa], (ch >> 1) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t bb = smem_u32(smem + PtSmem::OFF_B + sb * 2 * PT_BTILE);
-                const uint64_t b_hi = make_kmajor_desc<128>(bb), b_lo = make_kmajor_desc<128>(bb + PT_BTILE);
-#pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const uint32_t d = tmem_base + PT_TM_D + t * 80;
-                    const uint32_t a_hi = tmem_base + PT_TM_A + sa * 128 + t * 64, a_lo = a_hi + 32;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(d, a_hi + 8 * k, b_hi + 2 * k, idesc, (ch | k) != 0);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(d, a_hi + 8 * k, b_lo + 2 * k, idesc, 1);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16_ts(d, a_lo + 8 * k, b_hi + 2 * k, idesc, 1);
-                }
-                umma_commit(&a_empty[sa]);
-                umma_commit(&b_empty[sb]);
-                if (ch == nchunk - 1) umma_commit(d_full);
-            }
-            __syncwarp();
-        }
-    } else if (warp < PT_CW) {
-        // ===================== sigmoid / panoptic warps =====================
-        const int wq = warp & 3, qh = warp >> 2;              // TMEM lane quarter / which quarter (16 queries) of the chunk
-        const int dy = wq & 1, kyl = wq >> 1, dx = lane & 3, kxl = lane >> 2;
-        const int y_a = 4 * (ky0 + kyl) - 2 + dy, y_b = y_a + 2;
-        const int px = 4 * (kx0 + kxl) - 2 + dx;
-        const float lx1 = 0.125f + 0.25f * dx;
-        const float lya1 = 0.125f + 0.25f * dy, lyb1 = lya1 + 0.5f;
-        const bool xv = px >= 0 && px < Wc;
-        const bool pva = xv && y_a >= 0 && y_a < Hc, pvb = xv && y_b >= 0 && y_b < Hc;
-        const int tb = kyl * PP_TC + kxl;
-        const uint32_t tm = tmem_base + ((uint32_t)(wq * 32) << 16);
-        const int ctid = tid;                                 // 0..511 among the compute warps
-
-        // chunk-invariant staging offsets (512 threads cover 64 x 27 taps)
-        constexpr int NLD = (PP_QC * PP_TQ + PT_CT - 1) / PT_CT;
-        int goff[NLD];
-#pragma unroll
-        for (int k = 0; k < NLD; ++k) {
-            const int idx = ctid + k * PT_CT;
-            const int ql = idx / PP_TQ, rc = idx - ql * PP_TQ;
-            const int r = rc / PP_TC, c = rc - r * PP_TC;
-            const int yy = min(max(y_lo + r, 0), h - 1), xx = min(max(x_lo + c, 0), w - 1);
-            goff[k] = idx < PP_QC * PP_TQ ? (ql * h + yy) * w + xx : -1;
-        }
-        const size_t hw = (size_t)h * w;
-        float tv[NLD];
-        auto load_taps = [&](int q0) {
-#pragma unroll
-            for (int k = 0; k < NLD; ++k) {
-                const int ql = (ctid + k * PT_CT) / PP_TQ;
-                tv[k] = (goff[k] >= 0 && q0 + ql < Q) ? -1.4426950408889634f * __ldg(masks + (size_t)q0 * hw + goff[k]) : 1e30f;
-            }
-        };
-        auto store_taps = [&](int buf) {
-#pragma unroll
-            for (int k = 0; k < NLD; ++k) {
-                const int idx = ctid + k * PT_CT;
-                if (idx < PP_QC * PP_TQ) taps[buf * PP_QC * PP_TQ + idx] = tv[k];
-            }
-        };
-        // P^T chunk -> 128B-swizzled K-major tile: row = class (128 bytes = 64 queries), 16-byte chunk c of row r at c ^ (r & 7)
-        auto load_b = [&](int q0, int stage, int par) {
-            uint8_t* bt = smem + PtSmem::OFF_B + stage * 2 * PT_BTILE;
-            for (int i = ctid; i < 80 * 8; i += PT_CT) {
-                const int row = i >> 3, c = i & 7;
-                const int so = row * 128 + ((c ^ (row & 7)) << 4);
-                cp_async16(bt + so, pt_hi + (size_t)row * Qpad + q0 + c * 8);
-                cp_async16(bt + PT_BTILE + so, pt_lo + (size_t)row * Qpad + q0 + c * 8);
-            }
-            if (ctid < PP_QC / 4) cp_async16(sc + par * PP_QC + ctid * 4, scores + q0 + ctid * 4);   // scores: chunk parity
-            asm volatile("cp.async.commit_group;" ::: "memory");
-        };
-
-        float best_a = 0.f, best_b = 0.f;
-        int bidx_a = -1, bidx_b = -1;
-        load_taps(0);
-        load_b(0, 0, 0);
-        for (int ch = 0; ch < nchunk; ++ch) {
-            const int buf = ch & 1, q0 = ch * PP_QC, sb = ch % PT_NB;
-            store_taps(buf);
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
-            fence_proxy_async_smem();                          // cp.async / st.shared data -> visible to the tensor-core proxy
-            asm volatile("bar.sync 1, %0;" ::"n"(PT_CT) : "memory");     // taps(ch), B(ch), scores(ch) staged by all compute warps
-            if (ctid == 0) mbar_arrive(&b_full[sb]);
-            if (ch + 1 < nchunk) {
-                const int sn = (ch + 1) % PT_NB;
-                load_taps(q0 + PP_QC);
-                if (ch + 1 >= PT_NB) mbar_wait(&b_empty[sn], ((ch + 1) / PT_NB - 1) & 1);   // MMA of chunk ch+1-NB retired
-                load_b(q0 + PP_QC, sn, buf ^ 1);
-            }
-            const float* tp = taps + buf * PP_QC * PP_TQ + tb;
-            const float* scb = sc + buf * PP_QC;
-            if (ch >= 2) {
-                mbar_wait(&a_empty[buf], ((ch >> 1) - 1) & 1);  // MMA of chunk ch-2 has consumed this A stage
-                tc_fence_after();
-            }
-            uint32_t ha[8], la[8], hb[8], lb[8];
-            uint32_t npk[4];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {                      // query pair (2i, 2i+1) of this warp's 16 queries
-                float sa2[2], sb2[2];
-                uint32_t n2 = 0;
-#pragma unroll
-                for (int jj = 0; jj < 2; ++jj) {
-                    const int ql = qh * 16 + 2 * i + jj;
-                    const float* T = tp + ql * PP_TQ;
-                    const float s_q = scb[ql];
-                    const float t00 = T[0], t10 = T[PP_TC];
-                    const float top = fmaf(lx1, T[1] - t00, t00);
-                    const float bot = fmaf(lx1, T[PP_TC + 1] - t10, t10);
-                    const float d = bot - top;
-                    const float va = fmaf(lya1, d, top), vb = fmaf(lyb1, d, top);
-                    const float ea = rcp_approx(1.f + ex2_approx(va)), eb = rcp_approx(1.f + ex2_approx(vb));
-                    sa2[jj] = ea; sb2[jj] = eb;
-                    const float pa = ea * s_q, pb = eb * s_q;
-                    const bool ua = pa > best_a, ub = pb > best_b;
-                    best_a = ua ? pa : best_a; bidx_a = ua ? q0 + ql : bidx_a;
-                    best_b = ub ? pb : best_b; bidx_b = ub ? q0 + ql : bidx_b;
-                    n2 |= (((pva && va <= 0.f) ? 1u : 0u) + ((pvb && vb <= 0.f) ? 1u : 0u)) << (8 * jj);
-                }
-                split2(sa2[0], sa2[1], ha[i], la[i]);
-                split2(sb2[0], sb2[1], hb[i], lb[i]);
-                if (i & 1) npk[i >> 1] |= n2 << 16; else npk[i >> 1] = n2;
-            }
-            // counts of sigmoid >= .5 per query over the warp's 64 pixels: 4 queries per packed word
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                uint32_t v = npk[i];
-                v += __shfl_xor_sync(0xffffffffu, v, 16);
-                v += __shfl_xor_sync(0xffffffffu, v, 8);
-                v += __shfl_xor_sync(0xffffffffu, v, 4);
-                v += __shfl_xor_sync(0xffffffffu, v, 2);
-                v += __shfl_xor_sync(0xffffffffu, v, 1);
-                if (lane < 4) {
-                    const uint32_t n = (v >> (8 * lane)) & 0xffu;
-                    if (n) atomicAdd(&cnt[Qpad + q0 + qh * 16 + 4 * i + lane], (int)n);
-                }
-            }
-            const uint32_t acol = tm + PT_TM_A + buf * 128 + qh * 8;
-            tmem_st_32x32b_x4(acol, ha[0], ha[1], ha[2], ha[3]);           tmem_st_32x32b_x4(acol + 4, ha[4], ha[5], ha[6], ha[7]);
-            tmem_st_32x32b_x4(acol + 32, la[0], la[1], la[2], la[3]);      tmem_st_32x32b_x4(acol + 36, la[4], la[5], la[6], la[7]);
-            tmem_st_32x32b_x4(acol + 64, hb[0], hb[1], hb[2], hb[3]);      tmem_st_32x32b_x4(acol + 68, hb[4], hb[5], hb[6], hb[7]);
-            tmem_st_32x32b_x4(acol + 96, lb[0], lb[1], lb[2], lb[3]);      tmem_st_32x32b_x4(acol + 100, lb[4], lb[5], lb[6], lb[7]);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&a_full[buf]);
-        }
-        // ---- panoptic winner: merge the four query quarters (warps w, w+4, w+8, w+12 own the same pixels) ----
-        const int pslot = (wq * 32 + lane) * 2;
-        int* xchi = reinterpret_cast<int*>(xch);
-        if (qh > 0) {
-            const int base = ((qh - 1) * 256 + pslot) * 2;
-            xch[base] = best_a; xchi[base + 1] = bidx_a;
-            xch[base + 2] = best_b; xchi[base + 3] = bidx_b;
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(PT_CT) : "memory");
-        if (qh == 0) {
-            const int first = *s_first == 0x7fffffff ? -1 : *s_first;
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-                float bv = t ? best_b : best_a;
-                int bi = t ? bidx_b : bidx_a;
-#pragma unroll
-                for (int o = 0; o < 3; ++o) {                   // increasing query ranges: ties keep the lower index
-                    const float ov = xch[(o * 256 + pslot + t) * 2];
-                    const int oi = xchi[(o * 256 + pslot + t) * 2 + 1];
-                    if (oi >= 0 && (bi < 0 || ov > bv)) { bv = ov; bi = oi; }
-                }
-                const bool pv = t ? pvb : pva;
-                if (pv) {
-                    int in = 0;
-                    if (bi >= 0) in = bv >= 0.5f * scores[bi];
-                    else bi = first;
-                    const int y = t ? y_b : y_a;
-                    ids[(size_t)y * Wc + px] = bi < 0 ? -1 : 2 * bi + in;
-                    if (bi >= 0) {
-                        atomicAdd(&cnt[bi], 1);
-                        if (in) atomicAdd(&cnt[2 * Qpad + bi], 1);
-                    }
-                }
-            }
-        }
-        // ---- semantic tile: quarter-warps 0/1 drain D_A (classes 0-47 / 48-79), 2/3 drain D_B; lanes = 32 consecutive pixels ----
-        mbar_wait(d_full, 0);
-        tc_fence_after();
-        const int dt = qh >> 1;
-        const int yo = dt ? y_b : y_a;
-        const bool pvo = dt ? pvb : pva;
-        const size_t plane = (size_t)Hc * Wc;
-        const int cb = (qh & 1) ? 48 : 0, ce = (qh & 1) ? 80 : 48;
-        for (int c0 = cb; c0 < ce; c0 += 16) {
-            uint32_t o[16];
-            tmem_ld_32x32b_x16(tm + PT_TM_D + dt * 80 + c0, o);
-            tmem_ld_wait();
-            if (pvo) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i)
-                    if (c0 + i < C) sem[(size_t)(c0 + i) * plane + (size_t)yo * Wc + px] = __uint_as_float(o[i]);
-            }
-            __syncwarp();
-        }
-        tc_fence_before();
-        asm volatile("bar.sync 1, %0;" ::"n"(PT_CT) : "memory");
-        for (int i = ctid; i < 3 * Qpad; i += PT_CT) {
-            const int v = cnt[i];
-            const int a = i / Qpad, q = i - a * Qpad;
-            if (v && q < Q) atomicAdd(&areas[a * Q + q], v);
-        }
-    }
-    __syncthreads();
-    if (warp == PT_CW) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-static int launch_seg_post_tc(const float* masks, const void* pt_hi, const void* pt_lo, const float* scores, float* sem,
-                              int* ids, int* areas, int Q, int Qpad, int C, int h, int w, int Hc, int Wc, cudaStream_t st) {
-    const int smem = PtSmem::OFF_CNT + 3 * Qpad * 4 + 1024;
-    HIPIE_CHECK_ARG(smem <= 220 * 1024, "hipie_seg_postprocess: Q=%d needs %d B of shared memory", Q, smem);
-    HIPIE_ENSURE_SMEM(seg_post_tc_kernel, smem);
-    dim3 grid(((Wc + 2 + 3) / 4 + PP_BX - 1) / PP_BX, ((Hc + 2 + 3) / 4 + PP_BY - 1) / PP_BY);
-    seg_post_tc_kernel<<<grid, PT_THREADS, smem, st>>>(masks, (const __nv_bfloat16*)pt_hi, (const __nv_bfloat16*)pt_lo, scores,
-                                                      sem, ids, areas, Q, Qpad, C, h, w, Hc, Wc);
-    HIPIE_CHECK_LAUNCH();
-    return HIPIE_OK;
-}
 
 // Instance masks (hipie_img.py:1003-1007): bilinear x4 (align_corners=False) of the 1/4-resolution logits, sigmoid, > threshold,
 // crop -- one pass, one byte per pixel out.  Thread = 4 consecutive pixels of one 4x4 block row (they share the 4 taps).
@@ -649,9 +337,6 @@ extern "C" int hipie_seg_postprocess(const float* masks, const void* pt_hi, cons
                         Hc <= 4 * h && Wc <= 4 * w,
                     "hipie_seg_postprocess: bad sizes Q=%d Qpad=%d C=%d h=%d w=%d Hc=%d Wc=%d", Q, Qpad, C, h, w, Hc, Wc);
     HIPIE_CHECK_CUDA(cudaMemsetAsync(areas, 0, sizeof(int) * 3 * Q, (cudaStream_t)stream));
-    static const bool use_mma_sync = getenv("HIPIE_SEGPOST_MMA_SYNC") != nullptr;     // A/B switch for measurements
-    if (C <= 80 && !use_mma_sync)
-        return launch_seg_post_tc(masks, pt_hi, pt_lo, scores, sem, ids, areas, Q, Qpad, C, h, w, Hc, Wc, (cudaStream_t)stream);
     if (C <= 80)
         return launch_seg_post<10>(masks, pt_hi, pt_lo, scores, sem, ids, areas, Q, Qpad, C, h, w, Hc, Wc, (cudaStream_t)stream);
     return launch_seg_post<17>(masks, pt_hi, pt_lo, scores, sem, ids, areas, Q, Qpad, C, h, w, Hc, Wc, (cudaStream_t)stream);

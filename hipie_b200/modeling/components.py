@@ -1,4 +1,4 @@
-"""Registry-level components with the reference's constructor / forward contracts, each running on the B200 engine:
+"""Registry-level components with the reference's constructor / forward contracts, each running on the CUDA engine:
 
   BACKBONE_REGISTRY            D2ViT(cfg, input_shape)          /root/reference/projects/HIPIE/hipie/backbone/vit.py:378-467
   SEM_SEG_HEADS_REGISTRY       MaskDINOHead(cfg, input_shape)   hipie/models/maskdino/meta_arch/maskdino_head.py:21-82
@@ -34,7 +34,7 @@ class _EngineComponent(nn.Module):
         self.hp = hp
         self.device_ = torch.device(device)
         if self.device_.type != "cuda":
-            raise RuntimeError("hipie_b200 components run on a CUDA (sm_100a) device only; there is no CPU path")
+            raise RuntimeError("hipie_b200 components run on a CUDA (sm_90a) device only; there is no CPU path")
         full = P.random_state_dict(hp, seed=seed)
         self._keys = [k for k in full if k.startswith(self.prefix)]
         self._sd = OrderedDict((k[len(self.prefix):], full[k]) for k in self._keys)

@@ -1,7 +1,7 @@
-"""B200 engine: HIPIE's eval forward expressed over the C-ABI operators (hipie_b200.ops).
+"""CUDA engine: HIPIE's eval forward expressed over the C-ABI operators (hipie_b200.ops).
 
 Functional, driven by a flat weight dictionary under the reference's state_dict names.  Layout choices are
-B200-first rather than a translation of the reference modules:
+GPU-first rather than a translation of the reference modules:
   * activations are token-major / NHWC fp32 "residual streams"; everything that feeds a tensor-core GEMM is
     produced directly as bf16 hi/lo planes by the preceding kernel's epilogue (LayerNorm, GELU, attention …),
   * convolutions are GEMMs over NHWC rows (1x1: plain; kxk: im2col; ConvTranspose 2x2: GEMM + pixel shuffle),
@@ -9,7 +9,7 @@ B200-first rather than a translation of the reference modules:
   * sampling-offset and attention-weight linears of MSDeformAttn are one fused GEMM (N = 384) feeding the fused
     softmax+location+gather kernel; the value map is projected once per layer,
   * the mask-embed contraction runs transposed (M = H*W pixels, N = queries) so the NHWC pixel features are the
-    K-major A operand and the (Q, H, W) output is written coalesced straight from TMEM lanes.
+    K-major A operand and the (Q, H, W) output is written coalesced straight from the accumulator.
 torch is used for allocation, views and a few tiny input-independent / index ops (top-k, gather, sine tables).
 
 Reference call sites are cited next to each stage (H = /root/reference/projects/HIPIE/hipie).
@@ -147,7 +147,7 @@ class Engine:
         self._maps = {}
         self._bufs = {}
         self.bf16_value_map = False     # fast mode: MSDeformAttn value map stored as bf16
-        self.use_tc_attention = True    # tcgen05 flash attention for the global ViT blocks
+        self.use_tc_attention = True    # wgmma flash attention for the global ViT blocks
         self.attn_fp16 = True           # precision map (DESIGN.md 3): QK^T / PV / rel-pos of the ViT attention run as ONE fp16 MMA pass
         self.qkv_f16x2 = True           # ... and the qkv linears feeding it as TWO fp16 passes (LN output one fp16 plane, W fp16 hi + lo)
         self.fp16_value_map = False     # value maps of the deformable ENCODERS (Lq == S) as one fp16 plane (msda_layer): measured and REJECTED
@@ -215,7 +215,7 @@ class Engine:
                 Bq, Tq, qh, qw = B * nW, ws * ws, ws, ws
             else:
                 Bq, Tq, qh, qw = B, T, gh, gw
-            # tcgen05 kernel: 64-wide grids (1024-pixel inputs), 80-wide grids (1280-pixel inputs; T a multiple of lcm(256, 320)) and 14x14 windows
+            # wgmma kernel: 64-wide grids (1024-pixel inputs), 80-wide grids (1280-pixel inputs; T a multiple of lcm(256, 320)) and 14x14 windows
             tc_grid = Tq % 256 == 0 and (qw == 64 or (qw == 80 and Tq % 320 == 0))
             use_tc = self.use_tc_attention and hd == 80 and ((not windowed and tc_grid) or (windowed and ws == 14))
             f16 = use_tc and self.attn_fp16 and ops.PREC == 3

@@ -1,4 +1,4 @@
-"""HIPIE_IMG meta-architecture on the B200 engine — drop-in for the reference's
+"""HIPIE_IMG meta-architecture on the CUDA engine — drop-in for the reference's
 `META_ARCH_REGISTRY.get("HIPIE_IMG")(cfg)` (/root/reference/projects/HIPIE/hipie/hipie_img.py:45-420):
 same constructor argument (a cfg node), same `forward(batched_inputs, do_postprocess=True)` contract, same
 state_dict key names (modeling/params.py), same output dictionaries.
@@ -86,7 +86,7 @@ class HIPIE_IMG(nn.Module):
         self.hp = hp
         self.device_ = torch.device(device or (cfg.MODEL.DEVICE if cfg is not None else "cuda"))
         if self.device_.type != "cuda":
-            raise RuntimeError("hipie_b200.HIPIE_IMG runs on a CUDA (sm_100a) device only; there is no CPU path")
+            raise RuntimeError("hipie_b200.HIPIE_IMG runs on a CUDA (sm_90a) device only; there is no CPU path")
         self.demo_only = False
         self.num_bg, self.num_fg = hp.get("num_bg", 10), hp.get("num_queries", 900)
         self.mask_stride, self.mask_thres = hp.get("mask_stride", 4), hp.get("mask_thres", 0.5)
@@ -223,7 +223,7 @@ class HIPIE_IMG(nn.Module):
     def capture_hot_path(self, tensor, pad_mask, image_sizes, input_ids, attention_mask, task="detection", warmup=2, same_rows=None,
                          chunk_plan=None):
         """CUDA-graph the hot path (text encoder + coco_inference) for fixed-shape serving: ~2000 kernel launches per
-        batch become one graph launch, which removes the host launch overhead (B200: ≈15 % of the step).
+        batch become one graph launch, which removes the host launch overhead.
         Returns `replay() -> out` whose tensors are static buffers; refill `tensor` / `input_ids` in place between replays."""
         from .. import _lib
         ids, am = input_ids.to(self.device_), attention_mask.to(self.device_)

@@ -1,4 +1,4 @@
-"""MaskCLIP re-scoring on the B200 (SURVEY.md row a22 / f2).
+"""MaskCLIP re-scoring on the GPU (SURVEY.md row a22 / f2).
 
 Reference: projects/HIPIE/hipie/open_vocab/clip.py:243-383 (`MaskCLIP`: mask tokens = copies of the CLS token that attend to CLS and
 to the patches their mask touches; nobody attends to them), open_vocab/helper.py:79-130, hipie_img.py:811-868 (`get_clip_logits`)
@@ -38,7 +38,7 @@ def config_from_state_dict(sd):
 class MaskCLIP:
     def __init__(self, state_dict, device="cuda:0", cfg=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("hipie_b200 MaskCLIP: CUDA (sm_100a) only")
+            raise RuntimeError("hipie_b200 MaskCLIP: CUDA (sm_90a) only")
         self.device = torch.device(device)
         sd = {k: v.detach().to(self.device, torch.float32) for k, v in state_dict.items() if v.dtype.is_floating_point}
         self.cfg = dict(cfg) if cfg is not None else config_from_state_dict(sd)

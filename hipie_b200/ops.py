@@ -424,7 +424,7 @@ def attention(q: BF2, k: BF2, v: BF2, B, H, Tq, Tk, hd, q_strides, k_strides, v_
 
 def attention_tc(q: BF2, k: BF2, vt: BF2, B, H, T, hd, q_bs, q_ts, k_bs, k_ts, scale, rel_h=None, rel_w=None, kh=0, kw=0,
                  want_f32=False, want_split=True, prec=None, f16=False, out_e4m3=False):
-    """tcgen05 flash attention.  q, k: plane views whose row (token) holds all heads contiguously (head h at columns
+    """wgmma flash attention.  q, k: plane views whose row (token) holds all heads contiguously (head h at columns
     [80h, 80h+80) of the view); vt: BF2 (H*hd, B*T) = V transposed.  Output (B, T, H*hd)."""
     prec = PREC if prec is None else prec
     if f16:            # q / k / vt are single fp16 planes (gemm(out_fp16=True)); the output stays bf16 hi/lo for the 3-pass proj GEMM
@@ -554,8 +554,7 @@ def condinst_masks(feats_nhwc, params, ref_px, Hf, Wf, stride=8):
 def seg_postprocess(masks_low, cls_prob, threshold, Hc, Wc, stride=4):
     """Fused semantic + panoptic tensor work for one image (hipie_seg_postprocess).
     masks_low (Q,h,w) f32 logits, cls_prob (Q,C) f32.  Returns sem (C,Hc,Wc), ids (Hc,Wc) i32 [-1 | 2q+inter], areas (3,Q) i32,
-    scores (Q), labels (Q).  Any number of classes: vocabularies wider than one accumulator tile (80 classes on the tcgen05
-    kernel) run as class chunks of the same kernel, each writing its own rows of `sem`; the panoptic argmax / areas depend on the
+    scores (Q), labels (Q).  Any number of classes: vocabularies wider than one accumulator tile run as class chunks of the same kernel, each writing its own rows of `sem`; the panoptic argmax / areas depend on the
     per-query max over ALL classes only and are taken from the first chunk."""
     Q, h, w = masks_low.shape
     C = cls_prob.shape[1]

@@ -4,7 +4,7 @@ The reference's inference is pure data parallel: each rank owns a contiguous sha
 (/root/reference/detectron2/data/samplers/distributed_sampler.py:245-278 `InferenceSampler._get_local_indices`) and
 no collective is issued during the forward pass.  Here the global image batch is split the same way and the
 fixed-shape per-image outputs (class logits, boxes, MaskDINO logits, optionally bit-packed masks) are all-gathered
-once after the last kernel (NCCL over NVLink on the B200 box; gloo in the CPU tests).
+once after the last kernel (NCCL over NVLink between GPUs; gloo in the CPU tests).
 """
 from typing import Dict, List
 

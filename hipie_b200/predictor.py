@@ -1,4 +1,4 @@
-"""HIPIEPredictor on the B200 engine: same constructor and call signature as the reference's demo / evaluation predictor
+"""HIPIEPredictor on the CUDA engine: same constructor and call signature as the reference's demo / evaluation predictor
 (/root/reference/projects/HIPIE/predictor.py:245-372): takes one BGR uint8 image (cv2 layout), converts it per cfg.INPUT.FORMAT,
 applies ResizeShortestEdge(MIN_SIZE_TEST, MAX_SIZE_TEST), builds the caption and the label -> token map for the requested
 vocabulary (detection) or takes the referring expression (grounding), and runs `model([inputs])[0]`.

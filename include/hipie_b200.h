@@ -1,5 +1,5 @@
 /*
- * hipie_b200 — C-ABI of the B200-native HIPIE inference hot path.
+ * hipie_b200 — C-ABI of the H100-native (sm_90a) HIPIE inference hot path.
  *
  * Every entry point is `extern "C"`, takes plain device pointers + sizes + a
  * CUDA stream (passed as void*; NULL = legacy default stream), never
@@ -58,8 +58,7 @@ const char* hipie_last_error(void);
 int hipie_abi_version(void);
 /* Number of kernel launches issued through this library by the calling process. */
 int64_t hipie_launch_count(void);
-/* Process-wide tuning switches (tests / A-B measurements), all default 1.  "gemm_cta_pairs": large GEMMs run as CTA pairs
- * (tcgen05 cta_group::2, 256-row tiles), 0 forces single-CTA tiles; "gemm_tma_store": row-major outputs leave through TMA stores;
+/* Process-wide tuning switches (tests / A-B measurements), all default 1.  "gemm_tma_store": row-major outputs leave through TMA stores;
  * "gemm_fast_transposed": vectorised epilogue of the transposed fp16 plane (V^T); "ln_bulk": LayerNorm rows staged by bulk copies;
  * "ln_grid_cap": LayerNorm grid capped at the resident CTAs (rows grid-strided).  Unknown names return HIPIE_EINVAL. */
 int hipie_set_option(const char* name, int value);
@@ -92,7 +91,7 @@ int hipie_msda_fused_forward(const void* value, const int64_t* spatial_shapes,
                              int out_split_bf16, void* out_lo, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * tcgen05 GEMM:  C[M,N] = act( A[M,K] . W[N,K]^T + bias[N] ) * colscale[N] + residual[M,N]
+ * wgmma GEMM:  C[M,N] = act( A[M,K] . W[N,K]^T + bias[N] ) * colscale[N] + residual[M,N]
  * A and W are bf16 "split" operands: a_hi/a_lo and w_hi/w_lo (lo may be NULL when prec == 1).
  *   prec == 1 : C = Ahi.Whi                      (plain bf16, fp32 accumulate)
  *   prec == 3 : C = Ahi.Whi + Ahi.Wlo + Alo.Whi  (bf16x3 split, ~fp32 accuracy)
@@ -234,12 +233,12 @@ typedef struct hipie_attn_args {
 
 int hipie_attention(const hipie_attn_args* args, void* stream);
 
-/* tcgen05 flash attention for the ViT-H blocks (Attention.forward + add_decomposed_rel_pos, backbone/vit.py:67-83,
+/* wgmma flash attention for the ViT-H blocks (Attention.forward + add_decomposed_rel_pos, backbone/vit.py:67-83,
  * backbone/utils.py:96-125), hd == 80.  Two modes, selected by the shapes:
  *   global : T % 256 == 0, optional decomposed rel-pos bias with kw == 64 (1024-pixel inputs) or kw == 80 (1280-pixel inputs; then
- *            also T % 320 == 0), kh * kw == T; one CTA per 256 queries.  Other grids: HIPIE_EINVAL (callers use hipie_attention).
- *   window : T == 196 with kh == kw == 14 (the 14 x 14 windows; B = number of windows): one CTA per (window, head), the
- *            60 padding keys of the last 64-key tile are masked.
+ *            also T % 320 == 0), kh * kw == T; one CTA per 128 queries.  Other grids: HIPIE_EINVAL (callers use hipie_attention).
+ *   window : T == 196 with kh == kw == 14 (the 14 x 14 windows; B = number of windows): two CTAs of 128 query rows per
+ *            (window, head), the 60 padding query rows skip their stores and the 60 padding keys of the last 64-key tile are masked.
  * q / k are bf16 planes viewed as (B, T, width) rows (token stride *_ts, batch stride *_bs, head h at columns
  * [*_col0 + 80 h, +80)); vt is V transposed, (H*80, B*T) planes with row stride vt_ld (the qkv GEMM emits it with transposed=1);
  * in window mode every window sits at a 200-column pitch, (H*80, B*200), with zero pad columns (t_row_group = 196,
@@ -252,13 +251,6 @@ int hipie_attention_tc(const void* q_hi, const void* q_lo, int64_t q_bs, int64_t
                        int kh, int kw, float* out_f32, void* out_hi, void* out_lo, int64_t o_bs, int64_t o_ts, int B,
                        int H, int T, int hd, float scale, int prec, void* stream);
 
-/* Same, with an optional device buffer (32 key tiles x 2 query tiles x 8 slots of clock64 stamps of CTA (0,0,0)) for pipeline
- * debugging (tools/fa_trace.py). */
-int hipie_attention_tc_traced(const void* q_hi, const void* q_lo, int64_t q_bs, int64_t q_ts, int q_col0, int q_width,
-                              const void* k_hi, const void* k_lo, int64_t k_bs, int64_t k_ts, int k_col0, int k_width,
-                              const void* vt_hi, const void* vt_lo, int64_t vt_ld, const float* rel_h, const float* rel_w,
-                              int kh, int kw, float* out_f32, void* out_hi, void* out_lo, int64_t o_bs, int64_t o_ts, int B,
-                              int H, int T, int hd, float scale, int prec, long long* trace, void* stream);
 /* Same attention, output written as the operand planes of a prec-6 hipie_gemm (the proj linear, H:backbone/vit.py:82): out_f16
  * (B, T, H*hd) ONE fp16 plane and out_e4m3 (B*T, 2*H*hd) = [e4m3(h) | e4m3(2^10 (o - h))]; contiguous outputs (o_ts == H*hd). */
 int hipie_attention_tc_planes(const void* q_hi, const void* q_lo, int64_t q_bs, int64_t q_ts, int q_col0, int q_width,

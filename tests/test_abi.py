@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/hipie_b200.h declares.
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/hipie_b200.h declares.
 No compute calls (no GPU here)."""
 import os
 import re
@@ -48,10 +48,12 @@ def test_ops_refuse_cpu_tensors(lib):
         ops.split(torch.zeros(8))
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native(lib):
+    import shutil
     import subprocess
     so = os.path.join(ROOT, "hipie_b200", "libhipie_b200.so")
-    sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass, "tcgen05.mma missing from the GEMM"
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    sass = subprocess.run([cuobjdump, "-sass", so], capture_output=True, text=True).stdout
+    assert "HGMMA" in sass, "16-bit wgmma missing from the GEMM / attention"
+    assert "QGMMA" in sass, "e4m3 wgmma missing from the prec-6 GEMM"
     assert "UTMALDG" in sass, "TMA loads missing"
-    assert "LDTM" in sass, "tcgen05.ld missing"

@@ -1,6 +1,6 @@
 """GPU: whole-model parity at the BASELINE.json sizes, UNFORCED (no selection is pinned to the oracle's) and forced.
 
-Every case builds the CPU oracle (oracle/hipie_oracle, the restatement of the reference eval forward) and the B200 engine
+Every case builds the CPU oracle (oracle/hipie_oracle, the restatement of the reference eval forward) and the CUDA engine
 from the same seeded weights, runs both on the same seeded inputs and compares
 
   * the continuous outputs stage by stage (ViT residual stream after blocks 8/16/32, FPN features, encoder memory, fused

@@ -399,7 +399,7 @@ def test_attention_decomposed_relpos(ops, cuda):
 @pytest.mark.parametrize("prec", [3, 1])
 @pytest.mark.parametrize("with_rel", [True, False])
 def test_attention_tcgen05(ops, cuda, prec, with_rel):
-    """tcgen05/TMEM flash attention (global ViT-H blocks) vs fp64 softmax attention; V supplied transposed."""
+    """wgmma flash attention (global ViT-H blocks) vs fp64 softmax attention; V supplied transposed."""
     g = torch.Generator(device="cuda").manual_seed(21 + prec)
     B, H, hd, gh, gw = 2, 3, 80, 4, 64          # T = 256 tokens: 2 query tiles x 4 key tiles
     T, E = gh * gw, H * hd
@@ -475,7 +475,7 @@ def test_relpos_tc_global_grid(ops, cuda):
 
 @pytest.mark.parametrize("prec", [3, 1])
 def test_attention_tcgen05_window_mode(ops, cuda, prec):
-    """14x14-window mode of the tcgen05 attention kernel: 196 tokens per (window, head), keys padded to 4x64 and masked,
+    """14x14-window mode of the wgmma attention kernel: 196 tokens per (window, head), keys padded to 4x64 and masked,
     decomposed rel-pos bias rel_h[q, k // 14] + rel_w[q, k % 14]; vs fp64 softmax attention."""
     g = torch.Generator(device="cuda").manual_seed(31 + prec)
     B, H, hd, gh, gw = 5, 3, 80, 14, 14          # 5 windows

@@ -1,4 +1,4 @@
-"""GPU: MaskCLIP re-scoring (SURVEY a22 / f2) -- the support kernels against torch restatements of the reference lines, the B200
+"""GPU: MaskCLIP re-scoring (SURVEY a22 / f2) -- the support kernels against torch restatements of the reference lines, the GPU
 MaskCLIP engine against the fixture produced by the UNMODIFIED reference classes (tests/golden/ref_maskclip.pt, oracle/
 gen_golden_modules.py gen_maskclip) and the whole model with CLIP attached against the CPU oracle."""
 import pytest
@@ -141,7 +141,7 @@ def test_clip_fuse_modes(ops, cuda, agg, C):
 
 
 def test_maskclip_engine_matches_reference_fixture(cuda, golden_dir):
-    """The B200 MaskCLIP (tiny CLIP weights recreated by name) against what the reference's own MaskCLIP / get_clip_logits produced"""
+    """The GPU MaskCLIP (tiny CLIP weights recreated by name) against what the reference's own MaskCLIP / get_clip_logits produced"""
     import os
     from hipie_b200 import ops
     from hipie_b200.modeling.maskclip import MaskCLIP, class_tables, config_from_state_dict

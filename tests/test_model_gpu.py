@@ -1,4 +1,4 @@
-"""GPU: whole-model parity of the B200 engine against the CPU oracle on the tiny ViT configuration
+"""GPU: whole-model parity of the CUDA engine against the CPU oracle on the tiny ViT configuration
 (same code paths as ViT-H: windowed + global blocks with rel-pos interpolation, 4 levels, VL fusion, two-stage
 top-k, bg queries, MaskDINO branch, CondInst), same seeded weights and inputs.
 
@@ -233,7 +233,7 @@ def test_ragged_batch_padding_and_output_resize(cuda):
 
 
 def test_wide_image_uses_tcgen05_attention(cuda):
-    """128 x 1024 input -> 8 x 64 token grid: the global blocks take the tcgen05 flash-attention path (kw == 64, T % 128 == 0,
+    """128 x 1024 input -> 8 x 64 token grid: the global blocks take the wgmma flash-attention path (kw == 64, T % 128 == 0,
     V emitted transposed by the GEMM); rel-pos tables are interpolated 127 -> 15 along the height axis."""
     from hipie_oracle import hparams, synth
     from hipie_oracle.model import HipieOracle

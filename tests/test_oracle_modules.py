@@ -5,6 +5,7 @@ so every test also checks that the oracle module exposes exactly the reference's
 import copy
 import os
 
+import numpy as np
 import pytest
 import torch
 import torch.nn as nn
@@ -13,11 +14,39 @@ from hipie_oracle import detr, maskdino, vit
 from hipie_oracle.synth import fill_by_name_
 
 
+def _unpack(v):
+    """Fixtures keep 0/1 masks as packed bits ({"packed_bits_of_shape", "dtype", "bits"}): restored to the stored tensor."""
+    if isinstance(v, dict) and "packed_bits_of_shape" in v:
+        shape = v["packed_bits_of_shape"]
+        n = 1
+        for d in shape:
+            n *= d
+        bits = torch.from_numpy(np.unpackbits(v["bits"].numpy())[:n].copy())
+        return bits.reshape(shape).to(getattr(torch, v["dtype"]))
+    if isinstance(v, dict):
+        return {k: _unpack(x) for k, x in v.items()}
+    if isinstance(v, list):
+        return [_unpack(x) for x in v]
+    if isinstance(v, tuple):
+        return tuple(_unpack(x) for x in v)
+    return v
+
+
 def _load(golden_dir, name):
     p = os.path.join(golden_dir, name)
     if not os.path.exists(p):
         pytest.skip(f"{name} not generated")
-    return torch.load(p)
+    return _unpack(torch.load(p))
+
+
+def _close(actual, ref, atol):
+    """allclose against a stored reference tensor, or against a fixed seeded sample of its elements ({"sample_of_shape", "idx",
+    "values"}: large outputs are stored that way to keep the fixtures small)."""
+    if isinstance(ref, dict):
+        assert tuple(actual.shape) == tuple(ref["sample_of_shape"]), (actual.shape, ref["sample_of_shape"])
+        actual, ref = actual.reshape(-1)[ref["idx"].long()], ref["values"]
+    err = (actual - ref).abs().max()
+    assert torch.allclose(actual, ref, atol=atol), err
 
 
 def _same_keys(module, keys):
@@ -59,7 +88,7 @@ def test_transformer_forward_matches_reference(golden_dir):
     lang = {k: v.clone() for k, v in g["lang"].items()}
     with torch.no_grad():
         hs, memory, init_ref, inter_refs, lang_out, aux = tr(g["srcs"], g["masks"], g["poses"], lang)
-    assert torch.allclose(memory, g["memory"], atol=2e-5), (memory - g["memory"]).abs().max()
+    _close(memory, g["memory"], 2e-5)
     assert torch.allclose(lang_out["hidden"], g["lang_hidden"], atol=2e-5)
     assert torch.allclose(aux["enc_scores"], g["enc_cls"][..., 0], atol=2e-5)
     assert torch.allclose(init_ref, g["init_ref"], atol=1e-5)
@@ -88,14 +117,15 @@ def test_maskdino_encoder_decoder_match_reference(golden_dir):
     fill_by_name_(enc, g["enc_seed"])
     with torch.no_grad():
         mf, out0, ms = enc.forward_features(g["feats"])
-    assert torch.allclose(mf, g["mask_features"], atol=2e-5), (mf - g["mask_features"]).abs().max()
+    _close(mf, g["mask_features"], 2e-5)
+    assert len(ms) == len(g["multi_scale"])
     for a, b in zip(ms, g["multi_scale"]):
-        assert torch.allclose(a, b, atol=2e-5)
+        _close(a, b, 2e-5)
     dec = maskdino.MaskDINODecoder(hidden_dim=256, num_queries=7, nheads=8, dim_feedforward=48, dec_layers=3, mask_dim=256, num_classes=256).eval()
     _same_keys(dec, g["dec_keys"])
     fill_by_name_(dec, g["dec_seed"])
     with torch.no_grad():
-        out = dec(g["multi_scale"], g["mask_features"])
+        out = dec(ms, mf)          # the encoder outputs just checked against the reference's (the fixture keeps a sample of them)
     assert torch.allclose(out["pred_logits"], g["pred_logits"], atol=5e-5)
     assert torch.allclose(out["pred_boxes"], g["pred_boxes"], atol=1e-5)
     assert torch.allclose(out["interm_masks"], g["interm_masks"], atol=1e-4)
@@ -135,7 +165,7 @@ def test_bert_encoder_chunk_path_matches_reference(golden_dir):
         long = enc({"input_ids": g["ids"], "attention_mask": g["am"]}, sep=1012)
         short = enc({"input_ids": g["ids2"], "attention_mask": g["am2"]}, sep=1012)
     assert torch.allclose(short["hidden"], g["hidden_short"], atol=1e-5)
-    assert torch.allclose(long["hidden"], g["hidden_long"], atol=1e-5), (long["hidden"] - g["hidden_long"]).abs().max()
+    _close(long["hidden"], g["hidden_long"], 1e-5)
 
 
 def test_postprocessing_matches_reference_inference(golden_dir):
@@ -166,7 +196,7 @@ def test_postprocessing_matches_reference_inference(golden_dir):
             post = HipieOracle.segmentation_postprocess(inst, isz, oh, ow)
             assert torch.allclose(post["pred_boxes"], ref["post_boxes"], atol=1e-4)
             assert torch.equal(post["pred_masks"], ref["post_masks"]) and torch.equal(post["pred_classes"], ref["post_classes"])
-            assert torch.allclose(r["sem_seg"], ref["sem_seg"], atol=1e-5)
+            _close(r["sem_seg"], ref["sem_seg"], 1e-5)
             assert torch.equal(r["panoptic_seg"][0], ref["panoptic_seg"])
             assert r["panoptic_seg"][1] == ref["segments_info"] and len(ref["segments_info"]) > 0
 

@@ -29,7 +29,6 @@ print(f"copy   2 GiB: {ms:.3f} ms  {2*buf.numel()*4/ms/1e6:.0f} GB/s (read+write
 ms = timeit(lambda: torch.sum(src))
 print(f"read   2 GiB: {ms:.3f} ms  {buf.numel()*4/ms/1e6:.0f} GB/s (read only)")
 del buf, src
-_lib.set_option("gemm_cta_pairs", 0)
 for (M, N, K) in [(174080, 2048, 32), (174080, 2048, 256), (174080, 256, 256), (8 * 300, 65536, 256)]:
     a = torch.randn(M, K, device=dev)
     w = torch.randn(N, K, device=dev) * 0.05

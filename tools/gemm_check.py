@@ -1,5 +1,5 @@
-"""GPU smoke + A/B of the GEMM variants (run under `timeout`): CTA-pair (cta_group::2) tiles and the TMA-store epilogue against
-single-CTA tiles with the register-store epilogue.  Exit code 0 = every variant reproduces the baseline bit for bit on every
+"""GPU smoke + A/B of the GEMM epilogue variants (run under `timeout`): the TMA-store epilogue against the register-store
+epilogue.  Exit code 0 = every variant reproduces the baseline bit for bit on every
 case and agrees with an fp64 reference."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -9,11 +9,10 @@ from hipie_b200 import _lib, ops
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 ok = True
-VARIANTS = [(0, 0), (1, 0), (0, 1), (1, 1)]       # (pairs, tma_store); the first is the baseline
+VARIANTS = [0, 1]       # tma_store; the first is the baseline
 
 
-def setv(pairs, tma):
-    _lib.set_option("gemm_cta_pairs", pairs)
+def setv(tma):
     _lib.set_option("gemm_tma_store", tma)
 
 
@@ -33,8 +32,8 @@ for prec in (3, 1):
         res = torch.randn(M, N, device=dev) if kw.pop("res", False) else None
         cs = torch.rand(N, device=dev) + 0.5 if kw.pop("cs", False) else None
         outs = []
-        for pairs, tma in VARIANTS:
-            setv(pairs, tma)
+        for tma in VARIANTS:
+            setv(tma)
             f, s, bits = ops.gemm(A, W, prec=prec, bias=bias, residual=res, colscale=cs, **kw)
             torch.cuda.synchronize()
             outs.append((f, None if s is None else (s.hi, s.lo), bits))
@@ -76,8 +75,8 @@ for (M, N, K, kw) in [(32768, 5120, 1280, dict(act=ops.ACT_GELU, want_split=True
     a = torch.randn(M, K, device=dev)
     w = torch.randn(N, K, device=dev) * 0.05
     A, W = ops.split(a), ops.split_weight(w)
-    for pairs, tma in VARIANTS:
-        setv(pairs, tma)
+    for tma in VARIANTS:
+        setv(tma)
         for _ in range(3):
             ops.gemm(A, W, prec=3, **kw)
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -87,13 +86,13 @@ for (M, N, K, kw) in [(32768, 5120, 1280, dict(act=ops.ACT_GELU, want_split=True
         e.record()
         torch.cuda.synchronize()
         ms = s.elapsed_time(e) / 10
-        print(f"time pairs={pairs} tma={tma} {M}x{N}x{K} {'planes' if kw.get('want_split') else 'f32'}: {ms:.3f} ms  {2.0*M*N*K/ms/1e9:.0f} TF alg", flush=True)
+        print(f"time tma={tma} {M}x{N}x{K} {'planes' if kw.get('want_split') else 'f32'}: {ms:.3f} ms  {2.0*M*N*K/ms/1e9:.0f} TF alg", flush=True)
 # mask-embed shape (8 x (300 x 65536 x 256), fp32 rows + bits)
 me = torch.randn(8 * 300, 256, device=dev)
 px = torch.randn(8 * 65536, 256, device=dev)
 A, W = ops.split(me), ops.split_weight(px)
-for pairs, tma in VARIANTS:
-    setv(pairs, tma)
+for tma in VARIANTS:
+    setv(tma)
     fn = lambda: ops.gemm(A, W, M=300, N=65536, K=256, batch=8, lda=256, ldw=256, a_bstride=300 * 256, w_bstride=65536 * 256, bits_threshold=0.0, prec=3)
     for _ in range(3):
         fn()
@@ -105,7 +104,7 @@ for pairs, tma in VARIANTS:
     torch.cuda.synchronize()
     ms = s.elapsed_time(e) / 10
     alg = 8 * ((300 * 256 + 65536 * 256) * 4 + 300 * 65536 * 4 + 300 * 65536 / 8)
-    print(f"time pairs={pairs} tma={tma} mask-embed 8x(300x65536x256): {ms:.3f} ms  {alg/ms/1e6:.0f} GB/s algorithmic", flush=True)
-setv(1, 1)
+    print(f"time tma={tma} mask-embed 8x(300x65536x256): {ms:.3f} ms  {alg/ms/1e6:.0f} GB/s algorithmic", flush=True)
+setv(1)
 print("GEMM_CHECK_OK" if ok else "GEMM_CHECK_FAIL")
 sys.exit(0 if ok else 1)

@@ -1,7 +1,7 @@
 """CPU emulation of tensor-core operand formats on the oracle (experiment driver, test infrastructure).
 
 Rounds the operands of every nn.Linear / conv / ViT attention matmul to a 16-bit format before the fp32 product, which is
-what a one-pass tcgen05 kind::f16 contraction computes (exact products, fp32 accumulation), and reports how far the
+what a one-pass fp16 tensor-core contraction (wgmma) computes (exact products, fp32 accumulation), and reports how far the
 final outputs move from the plain fp32 oracle.  Used to choose the per-contraction precision map (DESIGN.md §3).
 """
 import argparse, os, sys, time

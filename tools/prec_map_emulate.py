@@ -2,7 +2,7 @@
 
 tools/prec_emulate.py rounds whole classes of contractions; this one takes rules `regex=A_FMT/W_FMT` over the oracle's module
 names (optional third field: format the OUTPUT is rounded to) (nn.Linear only) and rounds the activation / weight operand of the matching linears before the exact fp32 product:
-`f16/f16` is what ONE tcgen05 kind::f16 pass computes, `f16/-` a two-pass scheme (A in one fp16 plane, W in hi + lo planes),
+`f16/f16` is what ONE fp16 wgmma pass computes, `f16/-` a two-pass scheme (A in one fp16 plane, W in hi + lo planes),
 `-/f16` the other two-pass scheme.  The ViT attention itself (QK^T, P.V) always runs in the adopted fp16 mode here, so the
 numbers are increments on top of the shipped precision map (DESIGN.md 3).
 
