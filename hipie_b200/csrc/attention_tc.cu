@@ -9,7 +9,8 @@
 //                   16-wide box)
 //   warpgroups 1-2  64 query rows each: S = Q K^T (wgmma m64n64k16, both operands in shared memory), scale + rel-pos bias and the
 //                   online softmax on the register fragment, P packed in registers as the A operand of O += P V (wgmma m64n80k16,
-//                   A from registers), O in registers; the two warpgroups interleave on the tensor cores
+//                   A from registers), O in registers; S(j+1) is issued before the softmax of tile j, and the two warpgroups take
+//                   turns on the tensor cores (schedule at the key loop)
 //   window mode (T = 196, 14 x 14): keys padded to 4 x 64 and masked; V^T holds every window at a 200-column pitch because TMA
 //                   box starts must be 16-byte aligned
 // Precision: PREC==3 evaluates Qh.Kh + Qh.Kl + Ql.Kh and Ph.Vh + Ph.Vl + Pl.Vh (bf16x3, fp32-class); PREC==1 plain bf16 (or fp16).
@@ -26,6 +27,9 @@ int make_tmap_bf16(CUtensorMap* out, const void* ptr, int64_t rows, int64_t cols
 constexpr int FA_BM = 64, FA_BN = 64, FA_HD = 80, FA_STAGES = 3;
 constexpr int FA_CONSUMERS = 2;                        // consumer warpgroups per CTA, FA_BM query rows each
 constexpr int FA_THREADS = 128 * (1 + FA_CONSUMERS);   // + the producer warpgroup (one TMA thread)
+// setmaxnreg split of the 168 registers per thread of a 384-thread CTA: 24 + 2 x 240 = 3 x 168
+constexpr int FA_PRODUCER_REGS = 24, FA_CONSUMER_REGS = 240;
+constexpr int FA_BAR_TURN = 3;                         // named barriers 3, 4: tensor-core turn of consumer 0, 1 (1, 2: epilogue)
 constexpr int FA_OLD = FA_HD + 4;                      // row length (floats) of the staged output tile
 
 struct FaMaps {
@@ -126,6 +130,7 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
 
     if (warp < 4) {
         // ===================== TMA producer =====================
+        setmaxnreg_dec<FA_PRODUCER_REGS>();
         if (threadIdx.x == 0) {
             for (int c = 0; c < FA_CONSUMERS; ++c) {
                 uint8_t* qb = smem + SM::OFF_Q + c * SM::Q_TILE;
@@ -156,11 +161,15 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
         return;
     }
     // ===================== consumer warpgroup c: 64 query rows =====================
+    setmaxnreg_inc<FA_CONSUMER_REGS>();
     // wgmma fragment: this thread holds rows ra = 16 wq + lane / 4 and ra + 8, columns 8 j + 2 (lane % 4) + {0, 1}
     const int c = (threadIdx.x >> 7) - 1, wq = warp & 3, tig = lane & 3;
     const int ra = 16 * wq + (lane >> 2);
     const int qrow[2] = {q0 + c * FA_BM + ra, q0 + c * FA_BM + ra + 8};
     const bool has_rel = p.rel_h != nullptr;
+    // 64-wide grid: key tile j is key row j, so rel_h is one scalar per row and tile, and the key columns of this thread's
+    // fragment (rel_w) are the same in every tile. The 80-wide grid and the windows keep one rel_h + rel_w load per score.
+    constexpr bool ROW_TILES = !WIN && GW == FA_BN;
     const float* relw_row[2];
     const float* relh_row[2];
 #pragma unroll
@@ -169,44 +178,60 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
         relw_row[e] = has_rel ? p.rel_w + rowi * GW : nullptr;
         relh_row[e] = has_rel ? p.rel_h + rowi * (WIN ? FA_WIN : p.kh) : nullptr;
     }
+    float rw[2][16];                 // ROW_TILES: rel_w of row e at fragment column x (score index i: x = 2 (i / 4) + i % 2)
+    float rh[2] = {0.f, 0.f}, rh_next[2] = {0.f, 0.f};      // ROW_TILES: rel_h of the tile whose scores come next / the one after
+    if (ROW_TILES && has_rel) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+#pragma unroll
+            for (int x = 0; x < 16; ++x) rw[e][x] = __ldg(relw_row[e] + 8 * (x >> 1) + 2 * tig + (x & 1));
+            rh[e] = __ldg(relh_row[e]);
+            rh_next[e] = __ldg(relh_row[e] + (ntiles > 1 ? 1 : 0));
+        }
+    }
     constexpr float LOG2E = 1.4426950408889634f;
     const uint32_t qb = smem_u32(smem + SM::OFF_Q + c * SM::Q_TILE);
     float o[40];
 #pragma unroll
     for (int i = 0; i < 40; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};     // running max (log2 domain) / this thread's share of the row sum
-    mbar_wait(&q_full[c], 0);
-    for (int j = 0; j < ntiles; ++j) {
-        const int s = j % FA_STAGES;
-        const uint32_t par = (j / FA_STAGES) & 1;
-        // ---- S = Q K^T (PREC 3: Qh.Kh + Qh.Kl + Ql.Kh) ----
-        mbar_wait(&k_full[s], par);
-        float sacc[32];
-        const uint32_t kb = smem_u32(smem + s * SM::K_STAGE);
-        wg::fence();
+    float sacc[32];
+    float corr[2];
+    uint32_t pa_hi[4][4], pa_lo[4][4];
+
+    // ---- S = Q K^T of tile jt into sacc (PREC 3: Qh.Kh + Qh.Kl + Ql.Kh); the caller commits ----
+    auto issue_qk = [&](int jt) {
+        const uint32_t kb = smem_u32(smem + (jt % FA_STAGES) * SM::K_STAGE);
         fa_qk<F16>(sacc, qb, kb, SM::Q64, SM::K64, true);
         if (PREC == 3) {
             fa_qk<F16>(sacc, qb, kb + SM::K64 + SM::K16, SM::Q64, SM::K64, false);
             fa_qk<F16>(sacc, qb + SM::Q64 + SM::Q16, kb, SM::Q64, SM::K64, false);
         }
-        wg::commit();
-        wg::wait<0>();
-        wg::fence_regs(sacc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&k_empty[s]);
-        // ---- scores in the log2 domain: s * scale * log2e + (rel_h[q, key row] + rel_w[q, key column]) * log2e ----
+    };
+    // ---- O += P V from ring stage s (PREC 3: Ph.Vh + Ph.Vl + Pl.Vh); the caller commits ----
+    auto issue_pv = [&](int s) {
+        const uint32_t vb = smem_u32(smem + SM::OFF_V + s * SM::V_STAGE);
+        fa_pv<F16>(o, pa_hi, vb);
+        if (PREC == 3) {
+            fa_pv<F16>(o, pa_hi, vb + SM::VT);
+            fa_pv<F16>(o, pa_lo, vb);
+        }
+    };
+    // ---- scores of tile jt in the log2 domain, s * scale * log2e + (rel_h[q, key row] + rel_w[q, key column]) * log2e, the
+    //      online-softmax update of m and l, and exp2(t - m) in place. O is rescaled by corr later, once its PV has retired. ----
+    auto softmax = [&](int jt) {
         float tmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
             const int e = (i >> 1) & 1;
-            const int k = j * FA_BN + 8 * (i >> 2) + 2 * tig + (i & 1);
+            const int k = jt * FA_BN + 8 * (i >> 2) + 2 * tig + (i & 1);
             float t = sacc[i] * p.scale_log2e;
             if (WIN && k >= FA_WIN_T) t = -INFINITY;
-            else if (has_rel) t = fmaf(__ldg(relh_row[e] + k / GW) + __ldg(relw_row[e] + k % GW), LOG2E, t);
+            else if (ROW_TILES && has_rel) t = fmaf(rh[e] + rw[e][2 * (i >> 2) + (i & 1)], LOG2E, t);
+            else if (!ROW_TILES && has_rel) t = fmaf(__ldg(relh_row[e] + k / GW) + __ldg(relw_row[e] + k % GW), LOG2E, t);
             sacc[i] = t;
             tmax[e] = fmaxf(tmax[e], t);
         }
-        float corr[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             tmax[e] = fmaxf(tmax[e], __shfl_xor_sync(0xffffffffu, tmax[e], 1));
@@ -217,13 +242,17 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
             l[e] *= corr[e];
         }
 #pragma unroll
+        for (int i = 0; i < 32; ++i) sacc[i] = ex2_approx(sacc[i] - m[(i >> 1) & 1]);
+    };
+    // ---- O *= corr, then P packed as the register A operand of the PV wgmma (fragment of S == fragment of A, 16 keys per
+    //      k-step). Runs only after the previous PV has retired: it rewrites O and the A registers that PV reads. ----
+    auto rescale_pack = [&]() {
+#pragma unroll
         for (int i = 0; i < 40; ++i) o[i] *= corr[(i >> 1) & 1];
-        // ---- P = exp2(t - m) as the register A operand of the PV wgmma (fragment of S == fragment of A, 16 keys per k-step) ----
-        uint32_t pa_hi[4][4], pa_lo[4][4];
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
             const int e = (i >> 1) & 1;
-            const float e0 = ex2_approx(sacc[i] - m[e]), e1 = ex2_approx(sacc[i + 1] - m[e]);
+            const float e0 = sacc[i], e1 = sacc[i + 1];
             uint32_t hi, lo = 0u;
             if (PREC == 3) {
                 split2(e0, e1, hi, lo);
@@ -239,21 +268,67 @@ attn_tc_kernel(const __grid_constant__ FaMaps maps, const FaParams p) {
             pa_hi[i >> 3][(i >> 1) & 3] = hi;
             pa_lo[i >> 3][(i >> 1) & 3] = lo;
         }
-        // ---- O += P V (PREC 3: Ph.Vh + Ph.Vl + Pl.Vh) ----
-        mbar_wait(&v_full[s], par);
-        const uint32_t vb = smem_u32(smem + SM::OFF_V + s * SM::V_STAGE);
+    };
+
+    // Schedule: iteration j issues S(j+1) = Q K(j+1)^T and O += P(j) V(j) back to back, then computes the softmax of S(j+1)
+    // while PV(j) runs. The two warpgroups take turns issuing (named barriers FA_BAR_TURN + c), so that one warpgroup's
+    // softmax runs while the other's wgmmas occupy the tensor cores. Warpgroup 0 goes first: warpgroup 1 pre-arrives on its
+    // barrier and skips its last arrival, so every barrier phase completes.
+    mbar_wait(&q_full[c], 0);
+    mbar_wait(&k_full[0], 0);
+    wg::fence();
+    issue_qk(0);
+    wg::commit();
+    wg::wait<0>();
+    wg::fence_regs(sacc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&k_empty[0]);
+    softmax(0);
+    rescale_pack();
+    if (c == 1) named_bar_arrive(FA_BAR_TURN, 2 * 128);
+    // (no wgmma sits under a condition: ptxas serialises every wgmma of the kernel when one does, hence the peeled last tile)
+    for (int j = 0; j + 1 < ntiles; ++j) {
+        const int s = j % FA_STAGES, s1 = (j + 1) % FA_STAGES;
+        if (ROW_TILES && has_rel) {       // one tile ahead: the loads have a whole iteration to land
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                rh[e] = rh_next[e];
+                rh_next[e] = __ldg(relh_row[e] + (j + 2 < ntiles ? j + 2 : ntiles - 1));
+            }
+        }
+        mbar_wait(&k_full[s1], ((j + 1) / FA_STAGES) & 1);
+        mbar_wait(&v_full[s], (j / FA_STAGES) & 1);
+        named_bar_sync(FA_BAR_TURN + c, 2 * 128);
+        wg::fence_regs(sacc);
         wg::fence_regs(o);
         wg::fence();
-        fa_pv<F16>(o, pa_hi, vb);
-        if (PREC == 3) {
-            fa_pv<F16>(o, pa_hi, vb + SM::VT);
-            fa_pv<F16>(o, pa_lo, vb);
-        }
+        issue_qk(j + 1);
         wg::commit();
+        issue_pv(s);
+        wg::commit();
+        named_bar_arrive(FA_BAR_TURN + (c ^ 1), 2 * 128);
+        wg::wait<1>();                    // S(j+1) retired, PV(j) may still run
+        wg::fence_regs(sacc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&k_empty[s1]);
+        softmax(j + 1);
         wg::wait<0>();
         wg::fence_regs(o);
         __syncwarp();
         if (lane == 0) mbar_arrive(&v_empty[s]);
+        rescale_pack();
+    }
+    {   // last tile: O += P V
+        const int s = (ntiles - 1) % FA_STAGES;
+        mbar_wait(&v_full[s], ((ntiles - 1) / FA_STAGES) & 1);
+        named_bar_sync(FA_BAR_TURN + c, 2 * 128);
+        wg::fence_regs(o);
+        wg::fence();
+        issue_pv(s);
+        wg::commit();
+        if (c == 0) named_bar_arrive(FA_BAR_TURN + 1, 2 * 128);
+        wg::wait<0>();
+        wg::fence_regs(o);
     }
     // ---- epilogue: O / l, staged row-major so that one thread writes 16 consecutive columns of one row ----
     float* os = reinterpret_cast<float*>(smem + SM::OFF_O) + c * FA_BM * FA_OLD;
