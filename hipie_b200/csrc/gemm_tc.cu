@@ -6,13 +6,18 @@
 // mask-embed contraction einsum("bqc,bchw->bqhw") (.../maskdino/transformer_decoder/maskdino_decoder.py:520-529) with the
 // sigmoid-threshold fused as a bit-packed output.
 //
-// Structure (one CTA per SM, 384 threads, 128 x BN tiles, BN = 64 or 128):
+// Structure (one CTA per SM, 384 threads, 128 x BN tiles, BN = 64, 128 or 256):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor tiles of A / W into a 3-4 stage 128B/64B-swizzled
 //                   shared-memory ring, completion on mbarriers (expect_tx)
 //   warpgroups 1-2  consumers, 64 tile rows each: wgmma (m64 x BN x 16, both operands from shared memory) into fp32 register
-//                   accumulators, one k-block in flight; then the accumulator is staged row-major in shared memory and each warp
-//                   runs the epilogue on 32 rows x BN/2 columns: fused bias / activation / layer-scale / residual, fp32 + bf16-split +
-//                   bit-packed outputs, row-major through TMA stores where possible
+//                   accumulators, one k-block in flight, then the fused epilogue: bias / activation / layer-scale / residual,
+//                   fp32 + bf16-split / fp16 / fp16 + e4m3 + bit-packed outputs, row-major through TMA stores where possible.
+//   BN = 64 / 128:  the accumulator is staged row-major in shared memory and each warp runs the epilogue on 32 rows x BN/2
+//                   columns; this path also writes the transposed outputs (the attention's V^T) and the bit-packed mask.
+//   BN = 256:       the ViT-H linears (prec 4 and 6, row-major).  A quarter fewer operand bytes per flop than 128 x 128, so more of the
+//                   L2 -> shared-memory feed turns into tensor work.  128 accumulators per consumer thread (setmaxnreg: 40
+//                   producer + 2 x 232 consumer registers); the staged tile would take 132 KB, so each warp runs the epilogue
+//                   straight from its 16 fragment rows (epilogue_frag), and a 4-stage ring fits (48 KB stages for prec 6).
 //
 // Precision: operands are bf16 "split" planes.  prec==1 uses hi only; prec==3 computes
 // Ahi.Whi + Ahi.Wlo + Alo.Whi in the same fp32 accumulator (error ~2^-16 relative, i.e.
@@ -25,13 +30,15 @@
 // The cross terms are 2^-11 of the product, so the 2^-4 relative rounding of their e4m3 factors lands at 2^-15..2^-16 -- the
 // class of the bf16x3 scheme (tools/prec_map_emulate.py: mask logits unchanged at 1.4e-4) -- and both of them are ONE fp8
 // contraction over 2K: operand planes A8 = [e4m3(Ah) | e4m3(2^10 Al)] (M x 2K) and W8 = [e4m3(2^14 Wl) | e4m3(2^4 Wh)]
-// (N x 2K), the two slots interleaved in 32-column groups (common.cuh: e4m3_slot0) so that producers write 64-byte row segments.  Per tile the MMA warp first sweeps the fp8 planes (kind::f8f6f4, K = 32 per instruction: twice the rate of the
-// 16-bit kinds), accumulating 2^14 x the cross terms, then the fp16 planes, whose first MMA rescales the accumulator with the
-// instruction's scale-input-d immediate (D = A.B + D * 2^-14).  Two pass-equivalents instead of three, same operand bytes.
+// (N x 2K), the two slots interleaved in 32-column groups (common.cuh: e4m3_slot0) so that producers write 64-byte row segments.
+// Per tile the consumers first sweep the fp8 planes (m64nNk32 e4m3 wgmma: twice the rate of the 16-bit kinds), accumulating
+// 2^14 x the cross terms, scale the accumulator by 2^-14 in registers, then sweep the fp16 planes.  Two pass-equivalents
+// instead of three, same operand bytes.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 #include <string.h>
 
@@ -42,6 +49,8 @@ constexpr int GEMM_BM = 128;
 constexpr int GEMM_CONSUMERS = 2;                            // warpgroups, 64 accumulator rows each
 constexpr int GEMM_EPI_WARPS = 4 * GEMM_CONSUMERS;
 constexpr int GEMM_THREADS = 128 + 128 * GEMM_CONSUMERS;     // producer warpgroup (one TMA thread) + the consumer warpgroups
+// setmaxnreg split of the 168 registers per thread of the 128 x 256 tiles (128 fp32 accumulators per consumer thread): 40 + 2 x 232
+constexpr int GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
 constexpr int EPI_LD = 16;  // row length (floats) of the epilogue transpose buffer; 16-byte groups are XOR-swizzled by row
 constexpr int EPI_WARP_BYTES = 4096;   // per epilogue warp: one 32 x 32 fp32 TMA-store box (or a 32 x 32 bf16 hi box + lo box)
 
@@ -76,6 +85,7 @@ template <int PREC, int BN>
 struct GemmCfg {
     static constexpr bool P4 = PREC == 4;
     static constexpr bool P6 = PREC == 6;                    // fp16 hi.hi sweep + e4m3 sweep for the two cross terms (see the header comment)
+    static constexpr bool WIDE = BN == 256;                  // prec 4 / 6 only: epilogue from the register fragment, no staged tile
     static constexpr int BK = (PREC == 3 || P4) ? 32 : 64;   // elements per k-block of the 16-bit operands; BK*2 bytes == swizzle span
     static constexpr int BK8 = 128;                          // elements (= bytes) per k-block of the e4m3 sweep
     static constexpr int SWZ = BK * 2;
@@ -84,12 +94,13 @@ struct GemmCfg {
     static constexpr int A_PLANES = PREC == 3 ? 2 : 1, W_PLANES = (PREC == 3 || P4) ? 2 : 1;     // prec 6: one plane per sweep, same tile bytes
     static constexpr int STAGE = A_PLANES * A_TILE + W_PLANES * W_TILE;     // layout: A_hi | W_hi | (A_lo) | W_lo
     static constexpr int ACC_LD = BN + 4;                    // fp32 accumulator tile staged for the epilogue: padded rows, lane = row reads
-    static constexpr int ACC_BYTES = GEMM_BM * ACC_LD * 4;  //   are conflict-free
+    static constexpr int ACC_BYTES = WIDE ? 0 : GEMM_BM * ACC_LD * 4;  //   are conflict-free
     static constexpr int EPI_BYTES = GEMM_EPI_WARPS * EPI_WARP_BYTES;
     static constexpr int SMEM_BUDGET = 232448 - 1024 - 256 - EPI_BYTES - ACC_BYTES;      // 227 KB per CTA
     static constexpr int MAX_STAGES = 4;
     static constexpr int STAGES = SMEM_BUDGET / STAGE < MAX_STAGES ? SMEM_BUDGET / STAGE : MAX_STAGES;
     static_assert(STAGES >= 3, "pipeline too shallow");
+    static_assert(!WIDE || (STAGES == 4 && (P4 || P6)), "the 128 x 256 tiles run prec 4 / 6 on a 4-stage ring");
     static constexpr int SMEM = STAGES * STAGE + ACC_BYTES + EPI_BYTES + 256 + 1024;
 };
 
@@ -516,22 +527,169 @@ __device__ __forceinline__ void epilogue_transposed(const GemmParams& p, const f
     }
 }
 
-// issue the wgmmas of one k-block for this warpgroup's 64 rows (A rows offset inside the stage by `a_off` bytes)
-template <int PREC, int BN>
-__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t st, uint32_t a_off, bool f8, bool f16_ops, bool first) {
+// Row-major epilogue of the 128 x 256 tiles, straight from the wgmma register fragment (a staged fp32 copy of the tile would
+// need 132 KB of shared memory).  The warp owns rows [m0, m0 + 16) and the 256 columns from n0.  Per 32-column chunk the two
+// lanes of a pair swap half of their values (shfl.xor 1), so that every lane holds 4 consecutive columns of ONE row: lane
+// 4 r + q holds row r + 8 (q & 1), columns 4 (q >> 1) + {0..3} of each 8-column group.  Bias, activation, layer-scale, residual
+// and the output splits then run on float4s in the order of the staged epilogues above, so they write the same bits.
+// Aligned outputs without a residual or row map leave as 16 x 32 TMA-store boxes, through the two 2 KB halves of the warp's
+// staging buffer in turn (`half`); the others as 16-byte global stores, two lanes completing one 32-byte sector of a row.
+// The chunk loop stays rolled (an unrolled one is ~8x the code, and the instruction fetch then bounds the GELU epilogue): each
+// chunk reads acc[0, 16) and shifts the next chunk's values down, so every register index is a compile-time constant.
+template <int ACT>
+__device__ __forceinline__ void epilogue_frag(const GemmParams& p, const CUtensorMap* tm_f32, const CUtensorMap* tm_hi,
+                                              const CUtensorMap* tm_lo, float (&acc)[128], uint32_t sbuf, uint32_t& half,
+                                              int b, int m0, int n0, int lane) {
+    if (m0 >= p.M) return;          // warp-uniform: these 16 rows lie below the matrix
+    const int q = lane & 3, br = (lane >> 2) + 8 * (q & 1);     // row of this lane inside the 16-row box
+    const bool odd = q & 1;
+    const bool quick = p.act == HIPIE_ACT_QUICK_GELU;
+    const float alpha = p.alpha;
+    int64_t orow = -1;              // output row, -1: none (below the matrix, or a pad row of the row map)
+    if (m0 + br < p.M) orow = p.row_map ? p.row_map[(int64_t)b * p.M + m0 + br] : m0 + br;
+    const float* res_b = p.residual ? p.residual + (int64_t)b * p.r_bstride : nullptr;
+    float* cf_b = p.c_f32 ? p.c_f32 + (int64_t)b * p.c_bstride : nullptr;
+    __nv_bfloat16* chi_b = p.c_hi ? p.c_hi + (int64_t)b * p.c_bstride : nullptr;
+    __nv_bfloat16* clo_b = p.c_lo ? p.c_lo + (int64_t)b * p.c_bstride : nullptr;
+    const bool vec_ok = ((p.ldc & 3) == 0) && (!res_b || (p.ldr & 3) == 0);
+#pragma unroll 1
+    for (int ch = 0; ch < 8; ++ch) {
+        const int nb = n0 + 32 * ch;
+        if (nb >= p.N) break;       // warp-uniform
+        float4 x[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int i = 4 * j;              // d[i + {0,1}]: row r, columns 2q + {0,1};  d[i + {2,3}]: row r + 8
+            const float s0 = __shfl_xor_sync(0xffffffffu, odd ? acc[i] : acc[i + 2], 1);
+            const float s1 = __shfl_xor_sync(0xffffffffu, odd ? acc[i + 1] : acc[i + 3], 1);
+            x[j] = odd ? make_float4(s0, s1, acc[i + 2], acc[i + 3]) : make_float4(acc[i], acc[i + 1], s0, s1);
+        }
+#pragma unroll
+        for (int i = 0; i < 112; ++i) acc[i] = acc[i + 16];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int col = nb + 8 * j + 4 * (q >> 1);
+            const float4 bias = p.bias ? load4_guard(p.bias, col, p.N, 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+            x[j].x = act_apply_t<ACT>(fmaf(x[j].x, alpha, bias.x), quick);
+            x[j].y = act_apply_t<ACT>(fmaf(x[j].y, alpha, bias.y), quick);
+            x[j].z = act_apply_t<ACT>(fmaf(x[j].z, alpha, bias.z), quick);
+            x[j].w = act_apply_t<ACT>(fmaf(x[j].w, alpha, bias.w), quick);
+            if (p.colscale) {
+                const float4 cs = load4_guard(p.colscale, col, p.N, 1.f);
+                x[j].x *= cs.x; x[j].y *= cs.y; x[j].z *= cs.z; x[j].w *= cs.w;
+            }
+        }
+        if (p.tma_out) {
+            // f32 box: 128-byte rows, 16-byte group g of row r at g ^ (r & 7) (SWIZZLE_128B); fp16 / bf16 boxes: 64-byte rows, group c
+            // of row r at c ^ ((r >> 1) & 3) (SWIZZLE_64B); the e4m3 box: 64-byte rows [slot 0 | slot 1] of the chunk, swizzled the same
+#pragma unroll 1
+            for (int pass = (p.c_f32 ? 0 : 1); pass < (p.c_hi ? 2 : 1); ++pass) {
+                const uint32_t buf = sbuf + half * 2048;
+                if (lane == 0) bulk_wait_read1();      // the store that last read this half has finished reading it
+                __syncwarp();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int g = 2 * j + (q >> 1);       // 4-column group inside the 32-column chunk
+                    if (pass == 0) {
+                        sts128(buf + br * 128 + ((g ^ (br & 7)) << 4), __float_as_uint(x[j].x), __float_as_uint(x[j].y),
+                               __float_as_uint(x[j].z), __float_as_uint(x[j].w));
+                        continue;
+                    }
+                    const uint32_t sw = (br >> 1) & 3, off = br * 64 + ((j ^ sw) << 4) + ((q >> 1) << 3);
+                    uint2 hi, lo;
+                    if (p.c_e4m3) {
+                        uint32_t h8, l8;
+                        split4_f16_e4m3(x[j], hi, h8, l8);
+                        const uint32_t rb = buf + 1024 + br * 64 + 4 * (g & 3);
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rb + ((((g >> 2)) ^ sw) << 4)), "r"(h8) : "memory");
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rb + (((2 + (g >> 2)) ^ sw) << 4)), "r"(l8) : "memory");
+                    } else {
+                        split2m(x[j].x, x[j].y, hi.x, lo.x, p.c_fp16);
+                        split2m(x[j].z, x[j].w, hi.y, lo.y, p.c_fp16);
+                        if (p.c_lo) asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(buf + 1024 + off), "r"(lo.x), "r"(lo.y) : "memory");
+                    }
+                    asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(buf + off), "r"(hi.x), "r"(hi.y) : "memory");
+                }
+                fence_proxy_async_smem();      // generic-proxy writes -> visible to the TMA (async proxy)
+                __syncwarp();
+                if (lane == 0) {
+                    if (pass == 0) {
+                        tma_store_3d(tm_f32, buf, nb, m0, b);
+                    } else {
+                        tma_store_3d(tm_hi, buf, nb, m0, b);
+                        if (p.c_e4m3) tma_store_3d(tm_lo, buf + 1024, 2 * nb, m0, b);      // both slots of columns [nb, nb + 32)
+                        else if (p.c_lo) tma_store_3d(tm_lo, buf + 1024, nb, m0, b);
+                    }
+                    bulk_commit();
+                }
+                half ^= 1;
+            }
+            continue;
+        }
+        if (orow < 0) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int col = nb + 8 * j + 4 * (q >> 1);
+            if (col >= p.N) continue;
+            float4 v = x[j];
+            const int64_t off = orow * p.ldc + col;
+            if (col + 3 < p.N && vec_ok) {
+                if (res_b) {
+                    const float4 rv = *reinterpret_cast<const float4*>(res_b + orow * p.ldr + col);
+                    v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
+                }
+                if (p.relu_post) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+                if (cf_b) *reinterpret_cast<float4*>(cf_b + off) = v;
+                if (chi_b) {
+                    uint2 hi, lo;
+                    split2m(v.x, v.y, hi.x, lo.x, p.c_fp16);
+                    split2m(v.z, v.w, hi.y, lo.y, p.c_fp16);
+                    *reinterpret_cast<uint2*>(chi_b + off) = hi;
+                    if (clo_b) *reinterpret_cast<uint2*>(clo_b + off) = lo;
+                }
+                continue;
+            }
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                if (col + e >= p.N) break;
+                float xv = e == 0 ? v.x : (e == 1 ? v.y : (e == 2 ? v.z : v.w));
+                if (res_b) xv += res_b[orow * p.ldr + col + e];
+                if (p.relu_post) xv = fmaxf(xv, 0.f);
+                if (cf_b) cf_b[off + e] = xv;
+                if (chi_b) {
+                    if (p.c_fp16) {
+                        reinterpret_cast<__half*>(chi_b)[off + e] = __float2half_rn(xv);
+                    } else {
+                        const __nv_bfloat16 h = __float2bfloat16_rn(xv);
+                        chi_b[off + e] = h;
+                        if (clo_b) clo_b[off + e] = __float2bfloat16_rn(xv - __bfloat162float(h));
+                    }
+                }
+            }
+        }
+    }
+}
+
+// issue the wgmmas of one k-block for this warpgroup's 64 rows (A rows offset inside the stage by `a_off` bytes); F8: a k-block
+// of the e4m3 sweep of prec 6
+template <int PREC, int BN, bool F8>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t st, uint32_t a_off, bool f16_ops, bool first) {
     using Cfg = GemmCfg<PREC, BN>;
-    if (f8) {
+    if constexpr (F8) {
         // e4m3 sweep: 128-byte rows, 32 bytes along K per wgmma
         const uint64_t da = wg::desc<128>(st + a_off), dw = wg::desc<128>(st + Cfg::A_TILE);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            if (BN == 64) wg::ss_e4m3_n64(*reinterpret_cast<float(*)[32]>(&acc), da + 2 * k, dw + 2 * k, !(first && k == 0));
+            if constexpr (BN == 256) wg::ss_e4m3_n256(acc, da + 2 * k, dw + 2 * k, !(first && k == 0));
+            else if (BN == 64) wg::ss_e4m3_n64(*reinterpret_cast<float(*)[32]>(&acc), da + 2 * k, dw + 2 * k, !(first && k == 0));
             else wg::ss_e4m3_n128(*reinterpret_cast<float(*)[64]>(&acc), da + 2 * k, dw + 2 * k, !(first && k == 0));
         }
         return;
     }
     auto mma = [&](uint64_t da, uint64_t dw, int scale_d) {
-        if (f16_ops) {
+        if constexpr (BN == 256) {
+            wg::ss_f16_n256(acc, da, dw, scale_d);      // the wide tiles run prec 4 / 6: fp16 operands
+        } else if (f16_ops) {
             if (BN == 64) wg::ss_f16_n64(*reinterpret_cast<float(*)[32]>(&acc), da, dw, scale_d);
             else wg::ss_f16_n128(*reinterpret_cast<float(*)[64]>(&acc), da, dw, scale_d);
         } else {
@@ -598,6 +756,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 
     if (warp < 4) {
         // ===================== TMA producer (one thread) =====================
+        if constexpr (Cfg::WIDE) setmaxnreg_dec<GEMM_PRODUCER_REGS>();
         if (threadIdx.x == 0) {
             int s = 0;
             uint32_t ph = 0;
@@ -630,8 +789,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         }
     } else {
         // ===================== consumer warpgroups: wgmma mainloop + epilogue =====================
-        // warpgroup c owns rows [64 c, 64 c + 64) of the 128-row tile; the epilogue gives each of its warps 32 of those rows and half
-        // of the BN columns
+        // warpgroup c owns rows [64 c, 64 c + 64) of the 128-row tile; the staged epilogue gives each of its warps 32 of those rows and
+        // half of the BN columns, the wide one (epilogue_frag) the warp's 16 fragment rows and all 256 columns
+        if constexpr (Cfg::WIDE) setmaxnreg_inc<GEMM_CONSUMER_REGS>();
         const int c = (threadIdx.x >> 7) - 1;
         const int wq = warp & 3;
         const int ew = warp - 4;                              // 0..7
@@ -649,6 +809,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         const uint32_t a_off8 = (uint32_t)c * 64u * (uint32_t)Cfg::BK8;           // ... of the e4m3 A tile
         int s = 0;
         uint32_t ph = 0;
+        uint32_t half = 0;                                    // epilogue_frag: staging half of the next TMA-store box
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const int b = t / tiles_per_batch;
             const int r = t - b * tiles_per_batch;
@@ -657,19 +818,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
             int prev = -1;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const bool f8 = Cfg::P6 && kb < num_kb8;
-                if (Cfg::P6 && kb == num_kb8) {
-                    // the e4m3 sweep accumulated 2^14 x the cross terms: rescale before the fp16 sweep adds Ah.Wh
-                    wg::wait<0>();
-                    wg::fence_regs(acc);
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) acc[i] *= 0x1p-14f;
-                }
+            auto kblock = [&](auto f8, bool first) {
                 mbar_wait(&full_bar[s], ph);
                 wg::fence_regs(acc);
                 wg::fence();
-                gemm_kblock<PREC, BN>(acc, smem_u32(stage_base + s * Cfg::STAGE), f8 ? a_off8 : a_off, f8, p.f16_ops != 0, kb == 0);
+                gemm_kblock<PREC, BN, decltype(f8)::value>(acc, smem_u32(stage_base + s * Cfg::STAGE), f8 ? a_off8 : a_off, p.f16_ops != 0, first);
                 wg::commit();
                 wg::wait<1>();                                   // the previous k-block's wgmmas have read their stage
                 wg::fence_regs(acc);
@@ -679,11 +832,33 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
                 }
                 prev = s;
                 if (++s == STAGES) { s = 0; ph ^= 1; }
+            };
+            // two loops, so that no wgmma and no accumulator update sits under a condition: ptxas serialises every wgmma of the
+            // kernel otherwise
+            if constexpr (Cfg::P6) {
+                for (int kb = 0; kb < num_kb8; ++kb) kblock(std::true_type{}, kb == 0);
+                // the e4m3 sweep accumulated 2^14 x the cross terms: rescale before the fp16 sweep adds Ah.Wh
+                wg::wait<0>();
+                wg::fence_regs(acc);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[i] *= 0x1p-14f;
             }
+            for (int kb = num_kb8; kb < num_kb; ++kb) kblock(std::false_type{}, kb == 0);
             wg::wait<0>();
             wg::fence_regs(acc);
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            if constexpr (Cfg::WIDE) {
+                const int m0 = mt * GEMM_BM + c * 64 + wq * 16, n0 = nt * BN;
+                switch (p.act) {
+                    case HIPIE_ACT_RELU: epilogue_frag<HIPIE_ACT_RELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, acc, my_sbuf, half, b, m0, n0, lane); break;
+                    case HIPIE_ACT_GELU: epilogue_frag<HIPIE_ACT_GELU>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, acc, my_sbuf, half, b, m0, n0, lane); break;
+                    case HIPIE_ACT_QUICK_GELU:
+                    case HIPIE_ACT_SIGMOID: epilogue_frag<HIPIE_ACT_SIGMOID>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, acc, my_sbuf, half, b, m0, n0, lane); break;
+                    default: epilogue_frag<HIPIE_ACT_NONE>(p, &tm_c_f32, &tm_c_hi, &tm_c_lo, acc, my_sbuf, half, b, m0, n0, lane); break;
+                }
+                continue;
+            }
             // accumulator fragment -> staged tile (row-major, padded): d[4j + {0,1}] at (16 wq + lane / 4, 8 j + 2 (lane % 4)), +8 rows
             {
                 const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
@@ -869,10 +1044,11 @@ static int launch_gemm(const hipie_gemm_args* a, cudaStream_t st) {
     CUtensorMap tc_f32 = ta_hi, tc_hi = ta_hi, tc_lo = ta_hi;
     if (tma_out) {
         const int64_t cbs = a->batch > 1 ? a->c_bstride : (int64_t)a->M * a->ldc;
-        if (a->c_f32 && (rc = make_tmap(&tc_f32, a->c_f32, 4, a->M, a->N, a->ldc, a->batch, cbs, 32, 32))) return rc;
-        if (a->c_hi && (rc = make_tmap(&tc_hi, a->c_hi, 2, a->M, a->N, a->ldc, a->batch, cbs, 32, 32))) return rc;
-        if (a->c_lo && (rc = make_tmap(&tc_lo, a->c_lo, 2, a->M, a->N, a->ldc, a->batch, cbs, 32, 32))) return rc;
-        if (a->c8 && (rc = make_tmap(&tc_lo, a->c8, 1, a->M, 2 * (int64_t)a->N, a->ldc8, 1, 0, 32, 64))) return rc;
+        const int box_rows = Cfg::WIDE ? 16 : 32;      // rows per epilogue warp
+        if (a->c_f32 && (rc = make_tmap(&tc_f32, a->c_f32, 4, a->M, a->N, a->ldc, a->batch, cbs, box_rows, 32))) return rc;
+        if (a->c_hi && (rc = make_tmap(&tc_hi, a->c_hi, 2, a->M, a->N, a->ldc, a->batch, cbs, box_rows, 32))) return rc;
+        if (a->c_lo && (rc = make_tmap(&tc_lo, a->c_lo, 2, a->M, a->N, a->ldc, a->batch, cbs, box_rows, 32))) return rc;
+        if (a->c8 && (rc = make_tmap(&tc_lo, a->c8, 1, a->M, 2 * (int64_t)a->N, a->ldc8, 1, 0, box_rows, 64))) return rc;
     }
     GemmParams p;
     p.tma_out = tma_out ? 1 : 0;
@@ -919,6 +1095,7 @@ extern "C" int hipie_gemm(const hipie_gemm_args* a, void* stream) {
     HIPIE_CHECK_ARG(a->a_hi && a->w_hi, "hipie_gemm: a_hi / w_hi required");
     HIPIE_CHECK_ARG((a->prec >= 1 && a->prec <= 4) || a->prec == 6, "hipie_gemm: prec must be 1, 2, 3, 4 or 6 (got %d)", a->prec);
     HIPIE_CHECK_ARG(a->prec != 6 || a->K % 32 == 0, "hipie_gemm: prec 6 needs K %% 32 == 0 (the e4m3 planes interleave 32-column groups)");
+    HIPIE_CHECK_ARG(a->prec != 6 || (!a->transposed && !a->c_bits), "hipie_gemm: prec 6 writes row-major outputs without the bit-packed mask");
     HIPIE_CHECK_ARG(a->prec != 6 || (a->a8 && a->w8 && a->batch == 1 && a->lda8 % 16 == 0 && a->ldw8 % 16 == 0 && a->lda8 >= 2 * (int64_t)a->K &&
                                      a->ldw8 >= 2 * (int64_t)a->K),
                     "hipie_gemm: prec 6 needs the e4m3 planes a8 (M x 2K) / w8 (N x 2K) with 16-byte aligned row strides, batch 1");
@@ -938,10 +1115,16 @@ extern "C" int hipie_gemm(const hipie_gemm_args* a, void* stream) {
     HIPIE_CHECK_ARG(!a->c_row_map || !a->transposed, "hipie_gemm: c_row_map is not supported with transposed=1");
     cudaStream_t st = (cudaStream_t)stream;
     // 128 x 64 tiles for narrow outputs, 128 x 128 otherwise (the fp32 accumulator of a 64-row warpgroup is 64 registers per
-    // thread at N = 128; its staged copy for the epilogue is what bounds the tile width in shared memory)
+    // thread at N = 128; its staged copy for the epilogue is what bounds the tile width in shared memory).  The ViT linears run
+    // 128 x 256 tiles with the epilogue from registers: a quarter fewer operand bytes per flop, which is what feeds the tensor
+    // cores from L2 at these shapes.  prec 6 (row-major only) takes them for every N > 64, ragged N clipped by the TMA; prec 4
+    // keeps 128 x 128 for N < 256, the transposed V^T output and the bit-packed mask.
     const bool narrow = a->N <= 64;
-    if (a->prec == 6) return narrow ? launch_gemm<6, 64>(a, st) : launch_gemm<6, 128>(a, st);   // fp16 + e4m3 split (the large ViT linears)
-    if (a->prec == 4) return narrow ? launch_gemm<4, 64>(a, st) : launch_gemm<4, 128>(a, st);   // two-pass fp16 (the qkv linears)
+    if (a->prec == 6) return narrow ? launch_gemm<6, 64>(a, st) : launch_gemm<6, 256>(a, st);   // fp16 + e4m3 split (the large ViT linears)
+    if (a->prec == 4) {                                                                           // two-pass fp16 (the qkv linears)
+        if (narrow) return launch_gemm<4, 64>(a, st);
+        return (a->N >= 256 && !a->transposed && !a->c_bits) ? launch_gemm<4, 256>(a, st) : launch_gemm<4, 128>(a, st);
+    }
     // prec 1 (bf16) and prec 2 (fp16) share the single-plane kernels; the wgmma type differs
     if (a->prec == 3) return narrow ? launch_gemm<3, 64>(a, st) : launch_gemm<3, 128>(a, st);
     return narrow ? launch_gemm<1, 64>(a, st) : launch_gemm<1, 128>(a, st);

@@ -125,6 +125,8 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t sm
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed groups of this thread have finished READING their shared-memory source (it may be overwritten)
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... all but the most recent one (double-buffered staging: the other buffer may be overwritten)
+__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 // ... have completed (global writes performed)
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
