@@ -305,8 +305,11 @@ _gn_ws = {}
 
 def groupnorm_nhwc(x, gamma, beta, eps=1e-5, groups=32, relu=False, post_add=None, want_f32=True, want_split=False,
                    out_f32=None, y_bstride=None, add_bstride=None):
-    """x: (N, HW, C) fp32 contiguous."""
+    """x: (N, HW, C) fp32 contiguous.  y_bstride / add_bstride: batch strides (elements) of out_f32 / post_add when they are views
+    of larger buffers; the bf16 planes are always (N, HW, C), so a strided output takes want_split=False."""
     N, HW, C = x.shape
+    if want_split and y_bstride is not None and y_bstride != HW * C:
+        raise ValueError("groupnorm_nhwc: want_split writes (N, HW, C) planes and cannot follow y_bstride")
     dev = x.device
     key = (dev, N * groups, torch.cuda.current_stream(dev).cuda_stream)       # one workspace per stream: branches of the forward overlap
     ws = _gn_ws.get(key)

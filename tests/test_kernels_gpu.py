@@ -595,9 +595,10 @@ def test_sine_embed(ops, cuda):
 
 def test_gemm_row_major_bits_short_wide(ops, cuda):
     """short-and-wide batched GEMM (the mask-embed shape class: M = 300 queries = 3 M tiles with a ragged last one, N = pixels):
-    M-fastest tile order, fp32 rows + fused (x > 0) bit-packed along N"""
+    N = 1536 is 12 = 4 x 3 N tiles, the smallest width that runs the M-fastest tile order (launch_gemm: tiles_m <= 8 and
+    tiles_n >= 4 tiles_m); fp32 rows + fused (x > 0) bit-packed along N"""
     g = torch.Generator(device="cuda").manual_seed(77)
-    B, M, N, K = 2, 300, 1024, 256
+    B, M, N, K = 2, 300, 1536, 256
     a = torch.randn(B * M, K, device=cuda, generator=g)
     w = torch.randn(B * N, K, device=cuda, generator=g) * 0.1
     A, W = ops.split(a), ops.split(w)
