@@ -180,10 +180,10 @@ class Engine:
             self._maps[key] = torch.tensor(values, dtype=dtype, device=self.device)
         return self._maps[key]
 
-    def _zero_bf2(self, key, shape):
+    def _zero_planes(self, key, shape, fmt="bf16x2"):
+        """Zero-initialised planes cached per key (the bf16 default carries both planes whatever the precision mode)."""
         if key not in self._bufs:
-            self._bufs[key] = BF2(torch.zeros(shape, dtype=torch.bfloat16, device=self.device),
-                                  torch.zeros(shape, dtype=torch.bfloat16, device=self.device))
+            self._bufs[key] = BF2.zeros(shape, self.device, fmt)
         return self._bufs[key]
 
     # ------------------------------------------------------------ ViT backbone (H/backbone/vit.py:233-374)
@@ -250,12 +250,9 @@ class Engine:
             if windowed:
                 rows_w = B * nW * ws * ws
                 if qkv2:
-                    key = ("winln16", rows_w, E)
-                    if key not in self._bufs:
-                        self._bufs[key] = BF2(torch.zeros((rows_w, E), dtype=torch.float16, device=self.device), None)
-                    xn = self._bufs[key]                                      # pad rows stay exactly zero
+                    xn = self._zero_planes(("winln16", rows_w, E), (rows_w, E), "f16")       # pad rows stay exactly zero
                 else:
-                    xn = self._zero_bf2(("winln", rows_w, E), (rows_w, E))
+                    xn = self._zero_planes(("winln", rows_w, E), (rows_w, E))
                 ops.layernorm(x, W[blk + ".norm1.weight"], W[blk + ".norm1.bias"], 1e-6, row_map=tok2win, out_split=xn, out_fp16=qkv2)
             else:
                 _, xn, _ = ops.layernorm(x, W[blk + ".norm1.weight"], W[blk + ".norm1.bias"], 1e-6, out_fp16=qkv2)
@@ -274,24 +271,18 @@ class Engine:
                     # V^T per window at a 200-column pitch (TMA box starts must be 16-byte aligned; 196 is not a multiple of 8);
                     # the 4 pad columns of every window stay zero in this cached buffer
                     if f16:
-                        key = ("vtwin16", E, Bq)
-                        if key not in self._bufs:
-                            self._bufs[key] = BF2(torch.zeros((E, Bq * 200), dtype=torch.float16, device=self.device), None)
-                        vt = self._bufs[key]
+                        vt = self._zero_planes(("vtwin16", E, Bq), (E, Bq * 200), "f16")
                     else:
-                        vt = self._zero_bf2(("vtwin", E, Bq), (E, Bq * 200))
+                        vt = self._zero_planes(("vtwin", E, Bq), (E, Bq * 200))
                     ops.gemm(xn, wv, bias=bv, want_f32=False, transposed=True, ldc=Bq * 200, out_split=vt, t_row_group=Tq, t_row_pad=200 - Tq,
                              out_fp16=f16, prec=qprec)
                 else:
                     _, vt, _ = ops.gemm(xn, wv, bias=bv, want_f32=False, want_split=True, transposed=True, out_fp16=f16, prec=qprec)  # (E, B*T)
-                q = BF2(qk.hi[:, 0:E], None if qk.lo is None else qk.lo[:, 0:E])
-                k = BF2(qk.hi[:, E:], None if qk.lo is None else qk.lo[:, E:])
+                q, k = qk[:, 0:E], qk[:, E:]
                 st = (Tq * 2 * E, 2 * E, hd)
             else:
                 _, qkv, _ = ops.gemm(xn, wqkv, bias=bqkv, want_f32=False, want_split=True)
-                q = BF2(qkv.hi[:, 0:E], None if qkv.lo is None else qkv.lo[:, 0:E])
-                k = BF2(qkv.hi[:, E:2 * E], None if qkv.lo is None else qkv.lo[:, E:2 * E])
-                vv = BF2(qkv.hi[:, 2 * E:], None if qkv.lo is None else qkv.lo[:, 2 * E:])
+                q, k, vv = qkv[:, 0:E], qkv[:, E:2 * E], qkv[:, 2 * E:]
             if f16:
                 Rh = W.cached(("relh16", blk, qh), lambda: ops.split_weight_f16(_get_rel_pos_table(qh, qh, W[blk + ".attn.rel_pos_h"])))
                 Rw = W.cached(("relw16", blk, qw), lambda: ops.split_weight_f16(_get_rel_pos_table(qw, qw, W[blk + ".attn.rel_pos_w"])))
@@ -308,11 +299,9 @@ class Engine:
                                          kh=qh, kw=qw, f16=f16, out_e4m3=proj6)
             else:
                 _, ao = ops.attention(q, k, vv, Bq, nh, Tq, Tq, hd, st, st, st, hd ** -0.5, rel_h=rel_h, rel_w=rel_w, kh=qh, kw=qw)
+            ao = ao.view(Bq * Tq, E)
             if proj6:
-                ao = BF2(ao.hi.view(Bq * Tq, E), ao.lo.view(Bq * Tq, 2 * E))
                 wproj = W.cached(("proj68", blk), lambda: ops.split_f16_e4m3(W[blk + ".attn.proj.weight"], weight=True))
-            else:
-                ao = ao.view(Bq * Tq, E)
             pprec = 6 if proj6 else None
             if windowed:
                 ops.gemm(ao, wproj, bias=bproj, residual=x, out_f32=x, row_map=win2tok, out_rows=B * T, prec=pprec)
@@ -457,16 +446,15 @@ class Engine:
     def ffn_postnorm(self, x, x_s, prefix, n1, n2, l1="linear1", l2="linear2"):
         """x = LN(x + linear2(relu(linear1(x))))"""
         W = self.W
-        if x_s.lo is not None and x_s.lo.dtype == torch.uint8:      # fp16 + e4m3 planes (encoder layers): both linears on gemm prec 6
+        if x_s.fmt == "f16+e4m3":      # fp16 + e4m3 planes (encoder layers): both linears on gemm prec 6
             w1, b1, w2, b2 = W.cached(("ffn68", prefix), lambda: (ops.split_f16_e4m3(W[f"{prefix}.{l1}.weight"], weight=True), W[f"{prefix}.{l1}.bias"],
                                                                    ops.split_f16_e4m3(W[f"{prefix}.{l2}.weight"], weight=True), W[f"{prefix}.{l2}.bias"]))
-            _, h, _ = ops.gemm(x_s, w1, bias=b1, act=ops.ACT_RELU, want_f32=False, out_e4m3=True, prec=6)
-            y, _, _ = ops.gemm(h, w2, bias=b2, residual=x, prec=6)
-            return ops.layernorm(y, W[f"{prefix}.{n2}.weight"], W[f"{prefix}.{n2}.bias"], 1e-5, want_f32=True, want_split=True)[:2]
-        w1, b1 = W.lin(f"{prefix}.{l1}")
-        w2, b2 = W.lin(f"{prefix}.{l2}")
-        _, h, _ = ops.gemm(x_s, w1, bias=b1, act=ops.ACT_RELU, want_f32=False, want_split=True)
-        y, _, _ = ops.gemm(h, w2, bias=b2, residual=x)
+            prec, hidden = 6, dict(out_e4m3=True)
+        else:
+            (w1, b1), (w2, b2) = W.lin(f"{prefix}.{l1}"), W.lin(f"{prefix}.{l2}")
+            prec, hidden = None, dict(want_split=True)
+        _, h, _ = ops.gemm(x_s, w1, bias=b1, act=ops.ACT_RELU, want_f32=False, prec=prec, **hidden)
+        y, _, _ = ops.gemm(h, w2, bias=b2, residual=x, prec=prec)
         return ops.layernorm(y, W[f"{prefix}.{n2}.weight"], W[f"{prefix}.{n2}.bias"], 1e-5, want_f32=True, want_split=True)[:2]
 
     def encoder_layer(self, prefix, src, src_s, pos, ref, mask_flat, shapes_t, lsi_t, B, S, shapes_host=None):
@@ -494,9 +482,7 @@ class Engine:
                                                      W[prefix + ".self_attn.in_proj_bias"][2 * d:].contiguous()))
         _, qk, _ = ops.gemm(qk_s.view(B * Q, d), win[0], bias=win[1], want_f32=False, want_split=True)     # (B*Q, 512)
         _, v, _ = ops.gemm(tgt_s.view(B * Q, d), win[2], bias=win[3], want_f32=False, want_split=True)
-        qq = BF2(qk.hi[:, :d], None if qk.lo is None else qk.lo[:, :d])
-        kk = BF2(qk.hi[:, d:], None if qk.lo is None else qk.lo[:, d:])
-        _, ao = ops.attention(qq, kk, v, B, 8, Q, Q, 32, (Q * 2 * d, 2 * d, 32), (Q * 2 * d, 2 * d, 32), (Q * d, d, 32), 32 ** -0.5)
+        _, ao = ops.attention(qk[:, :d], qk[:, d:], v, B, 8, Q, Q, 32, (Q * 2 * d, 2 * d, 32), (Q * 2 * d, 2 * d, 32), (Q * d, d, 32), 32 ** -0.5)
         wo, bo = W.lin(prefix + ".self_attn.out_proj")
         y, _, _ = ops.gemm(ao.view(B * Q, d), wo, bias=bo, residual=tgt.view(B * Q, d))
         t, t_s, _ = ops.layernorm(y, W[prefix + ".norm2.weight"], W[prefix + ".norm2.bias"], 1e-5, want_f32=True, want_split=False)
@@ -562,9 +548,8 @@ class Engine:
             p = f"{te}.encoder.layer.{i}"
             wqkv, bqkv = W.lin_cat(p + ".qkv", [p + ".attention.self.query", p + ".attention.self.key", p + ".attention.self.value"])
             _, qkv, _ = ops.gemm(x_s, wqkv, bias=bqkv, want_f32=False, want_split=True)
-            sl = lambda a, c: BF2(a.hi[:, c * Hd:(c + 1) * Hd], None if a.lo is None else a.lo[:, c * Hd:(c + 1) * Hd])
             st = (L * 3 * Hd, 3 * Hd, hd)
-            _, ao = ops.attention(sl(qkv, 0), sl(qkv, 1), sl(qkv, 2), R, nh, L, L, hd, st, st, st, hd ** -0.5, key_bias=key_bias)
+            _, ao = ops.attention(qkv[:, :Hd], qkv[:, Hd:2 * Hd], qkv[:, 2 * Hd:], R, nh, L, L, hd, st, st, st, hd ** -0.5, key_bias=key_bias)
             wo, bo = W.lin(p + ".attention.output.dense")
             y, _, _ = ops.gemm(ao.view(R * L, Hd), wo, bias=bo, residual=x)
             x, x_s, _ = ops.layernorm(y, W[p + ".attention.output.LayerNorm.weight"], W[p + ".attention.output.LayerNorm.bias"], 1e-12,
@@ -701,21 +686,16 @@ class Engine:
         # additive text mask: valid tokens +1, invalid -9e15 (fuse_helper.py:96-107)
         am = lang_mask.float()
         colbias = torch.where(am == 0, torch.full_like(am, -9e15), am).contiguous()
-        out_v = BF2(torch.empty(B * S, E, dtype=torch.bfloat16, device=self.device),
-                    torch.empty(B * S, E, dtype=torch.bfloat16, device=self.device) if ops.PREC == 3 else None)
-        out_l = BF2(torch.empty(B * Lt, E, dtype=torch.bfloat16, device=self.device),
-                    torch.empty(B * Lt, E, dtype=torch.bfloat16, device=self.device) if ops.PREC == 3 else None)
-        sub = lambda a, r0, r1, c0, c1: BF2(a.hi[r0:r1, c0:c1], None if a.lo is None else a.lo[r0:r1, c0:c1])
+        out_v, out_l = BF2.empty((B * S, E), self.device), BF2.empty((B * Lt, E), self.device)
         # the text->image P.V contraction runs over K = S pixels; TMA rows need 16-byte strides, i.e. a pixel count that is a multiple
         # of 8.  Image sizes whose level sum is not (e.g. 192 x 256 -> S = 1020) get zero-padded operand pitches (zeros add nothing).
         Sp = (S + 7) // 8 * 8
-        padS = lambda a, rows: a if Sp == S else BF2(F.pad(a.hi.reshape(rows, -1, S), (0, Sp - S)).reshape(rows, -1),
-                                                     None if a.lo is None else F.pad(a.lo.reshape(rows, -1, S), (0, Sp - S)).reshape(rows, -1))
+        padS = lambda a, rows: a.map(lambda t: F.pad(t.reshape(rows, -1, S), (0, Sp - S)).reshape(rows, -1))
         if Sp != S:
             vvT = padS(vvT, E)                                   # (E, B*Sp): every image at an Sp pitch
         for h in range(nh):
             c0, c1 = h * hd, (h + 1) * hd
-            qh, kh = sub(q_s, 0, B * S, c0, c1), sub(k_s, 0, B * Lt, c0, c1)
+            qh, kh = q_s[:, c0:c1], k_s[:, c0:c1]
             # scores (B, S, Lt) and its transpose (B, Lt, S): two GEMMs instead of a transpose pass
             sc, _, _ = ops.gemm(qh, kh, M=S, N=Lt, K=hd, batch=B, lda=E, ldw=E, a_bstride=S * E, w_bstride=Lt * E, prec=aprec)
             scT, _, _ = ops.gemm(kh, qh, M=Lt, N=S, K=hd, batch=B, lda=E, ldw=E, a_bstride=Lt * E, w_bstride=S * E, prec=aprec)
@@ -724,33 +704,15 @@ class Engine:
             if Sp != S:
                 pl = padS(pl, B * Lt)                            # (B*Lt, Sp)
             # out_v[b, s, c0:c1] = P_v[b] (S x Lt) . value_l[b]^T ; value_l^T rows c0:c1 of vlT, cols b*Lt..
-            ov = BF2(out_v.hi[:, c0:c1], None if out_v.lo is None else out_v.lo[:, c0:c1])
-            ol = BF2(out_l.hi[:, c0:c1], None if out_l.lo is None else out_l.lo[:, c0:c1])
-            self._gemm_into(pv, sub(vlT, c0, c1, 0, B * Lt), ov, M=S, N=hd, K=Lt, batch=B, lda=Lt, ldw=B * Lt, a_bstride=S * Lt,
-                            w_bstride=Lt, ldc=E, c_bstride=S * E, prec=aprec)
-            self._gemm_into(pl, sub(vvT, c0, c1, 0, B * Sp), ol, M=Lt, N=hd, K=Sp, batch=B, lda=Sp, ldw=B * Sp, a_bstride=Lt * Sp,
-                            w_bstride=Sp, ldc=E, c_bstride=Lt * E, prec=aprec)
+            ops.gemm(pv, vlT[c0:c1], want_f32=False, out_split=out_v[:, c0:c1], M=S, N=hd, K=Lt, batch=B, lda=Lt, ldw=B * Lt,
+                     a_bstride=S * Lt, w_bstride=Lt, ldc=E, c_bstride=S * E, prec=aprec)
+            ops.gemm(pl, vvT[c0:c1], want_f32=False, out_split=out_l[:, c0:c1], M=Lt, N=hd, K=Sp, batch=B, lda=Sp, ldw=B * Sp,
+                     a_bstride=Lt * Sp, w_bstride=Sp, ldc=E, c_bstride=Lt * E, prec=aprec)
         wov, bov = W.lin(p + ".attn.out_v_proj")
         wol, bol = W.lin(p + ".attn.out_l_proj")
         new_v, new_v_s, _ = ops.gemm(out_v, wov, bias=bov, colscale=W[p + ".gamma_v"], residual=v, want_split=True)
         new_l, _, _ = ops.gemm(out_l, wol, bias=bol, colscale=W[p + ".gamma_l"], residual=l)
         return new_v.view(B, S, 256), new_v_s.view(B, S, 256), new_l.view(B, Lt, Ld)
-
-    @staticmethod
-    def _gemm_into(a, w, out: BF2, **kw):
-        """GEMM whose bf16-split output lands in a strided view `out` (used to assemble multi-head outputs)."""
-        import ctypes
-        from .. import _lib
-        prec = kw.get("prec", ops.PREC)
-        args = _lib.GemmArgs(a_hi=a.hi.data_ptr(), a_lo=a.lo.data_ptr() if (a.lo is not None and prec == 3) else None,
-                             lda=kw["lda"], a_bstride=kw["a_bstride"], w_hi=w.hi.data_ptr(),
-                             w_lo=w.lo.data_ptr() if (w.lo is not None and prec == 3) else None, ldw=kw["ldw"], w_bstride=kw["w_bstride"],
-                             bias=None, colscale=None, residual=None, ldr=0, r_bstride=0, c_f32=None, c_hi=out.hi.data_ptr(),
-                             c_lo=out.lo.data_ptr() if out.lo is not None else None, ldc=kw["ldc"], c_bstride=kw["c_bstride"],
-                             c_bits=None, bits_threshold=0.0, M=kw["M"], N=kw["N"], K=kw["K"], batch=kw["batch"], act=0, prec=prec,
-                             alpha=1.0, transposed=0, c_row_map=None, t_row_group=0, t_row_pad=0, relu_after_residual=0, c_fp16=0)
-        _lib.check(_lib.load().hipie_gemm(ctypes.byref(args), ops._stream()), "gemm")
-
 
     # ------------------------------------------------------------ DETR: input projections + transformer + heads
     def detr_inputs(self, feats, pad_mask, B, any_pad=True):
@@ -855,9 +817,7 @@ class Engine:
         alpha = W.cached(("vl_alpha", prefix), lambda: float(1.0 / W[prefix + ".log_scale"].exp()))
         outs = []
         for b in range(B):       # per-image column bias; B tiny GEMMs (Q x Lt x 256)
-            a = BF2(q_s.hi[b * Q:(b + 1) * Q], None if q_s.lo is None else q_s.lo[b * Q:(b + 1) * Q])
-            w = BF2(tok_s.hi[b * Lt:(b + 1) * Lt], None if tok_s.lo is None else tok_s.lo[b * Lt:(b + 1) * Lt])
-            lg, _, _ = ops.gemm(a, w, bias=bias[b].contiguous(), alpha=alpha)
+            lg, _, _ = ops.gemm(q_s[b * Q:(b + 1) * Q], tok_s[b * Lt:(b + 1) * Lt], bias=bias[b].contiguous(), alpha=alpha)
             outs.append(lg)
         return torch.stack(outs, 0).clamp(min=-50000, max=50000)
 

@@ -16,7 +16,6 @@ import math
 import torch
 
 from .. import ops
-from ..ops import BF2
 
 OPENAI_MEAN = (0.48145466, 0.4578275, 0.40821073)
 OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -89,11 +88,10 @@ class MaskCLIP:
         for blk in blocks:
             _, xn, _ = ops.layernorm(x, blk["ln1"][0], blk["ln1"][1], 1e-5)
             _, qkv, _ = ops.gemm(xn, blk["qkv"][0], bias=blk["qkv"][1], want_f32=False, want_split=True)             # (B*T, 3 width)
-            sl = lambda c, r0: BF2(qkv.hi[r0:, c * width:(c + 1) * width], None if qkv.lo is None else qkv.lo[r0:, c * width:(c + 1) * width])
+            sl = lambda c, r0: qkv[r0:, c * width:(c + 1) * width]
             st = (T * 3 * width, 3 * width, hd)
             _, ao = ops.attention(sl(0, 0), sl(1, kv_row0), sl(2, kv_row0), B, heads, T, Tk, hd, st, st, st, hd ** -0.5, key_mask=key_mask)
-            ops.gemm(ao.view(B * T, width) if isinstance(ao, torch.Tensor) else BF2(ao.hi.view(B * T, width), None if ao.lo is None else ao.lo.view(B * T, width)),
-                     blk["out"][0], bias=blk["out"][1], residual=x, out_f32=x)
+            ops.gemm(ao.view(B * T, width), blk["out"][0], bias=blk["out"][1], residual=x, out_f32=x)
             _, xn2, _ = ops.layernorm(x, blk["ln2"][0], blk["ln2"][1], 1e-5)
             _, hmid, _ = ops.gemm(xn2, blk["fc"][0], bias=blk["fc"][1], act=ops.ACT_QUICK_GELU, want_f32=False, want_split=True)
             ops.gemm(hmid, blk["proj"][0], bias=blk["proj"][1], residual=x, out_f32=x)

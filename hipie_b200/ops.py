@@ -84,52 +84,96 @@ def _p(t: Optional[torch.Tensor]):
 
 
 class BF2:
-    """bf16 hi/lo planes of an fp32 tensor (lo is None in plain-bf16 mode)."""
+    """The operand planes of a tensor-core contraction: `hi` and an optional second plane `lo`.  The plane dtypes ARE the format
+    (DESIGN.md 2-3); this class is the one place that knows which pairs exist and how the second plane is shaped:
+
+        fmt          hi             lo               read by
+        "bf16"       bf16           None             gemm prec 1
+        "bf16x2"     bf16           bf16             gemm prec 3
+        "f16"        fp16           None             gemm prec 2, the A operand of prec 4, attention_tc(f16=True)
+        "f16x2"      fp16           fp16             the W operand of gemm prec 4, relpos_bias_tc_f16
+        "f16+e4m3"   fp16 (.., K)   uint8 (.., 2K)   gemm prec 6; lo holds two e4m3 slots per element, interleaved in 32-column groups
+    """
 
     __slots__ = ("hi", "lo")
+
+    _PLANES = {"bf16": (torch.bfloat16, None), "bf16x2": (torch.bfloat16, torch.bfloat16), "f16": (torch.float16, None),
+               "f16x2": (torch.float16, torch.float16), "f16+e4m3": (torch.float16, torch.uint8)}
+    _FMT = {v: k for k, v in _PLANES.items()}
 
     def __init__(self, hi, lo=None):
         self.hi, self.lo = hi, lo
 
     @property
+    def fmt(self):
+        pair = (self.hi.dtype, None if self.lo is None else self.lo.dtype)
+        if pair not in self._FMT:
+            raise TypeError(f"BF2: no plane format has hi {pair[0]} with lo {pair[1]}")
+        return self._FMT[pair]
+
+    @staticmethod
+    def _lo_shape(fmt, shape):
+        """Shape of the second plane for the logical shape (.., K): two e4m3 slots per element, otherwise the same."""
+        return tuple(shape[:-1]) + (2 * shape[-1],) if fmt == "f16+e4m3" else tuple(shape)
+
+    @classmethod
+    def empty(cls, shape, device, fmt=None, make=torch.empty):
+        """Uninitialised planes of the logical shape (.., K); fmt None: the bf16 planes of the current precision mode."""
+        fmt = ("bf16x2" if PREC == 3 else "bf16") if fmt is None else fmt
+        dhi, dlo = cls._PLANES[fmt]
+        hi = make(tuple(shape), dtype=dhi, device=device)
+        return cls(hi, None if dlo is None else make(cls._lo_shape(fmt, shape), dtype=dlo, device=device))
+
+    @classmethod
+    def zeros(cls, shape, device, fmt=None):
+        return cls.empty(shape, device, fmt, make=torch.zeros)
+
+    @property
     def shape(self):
         return self.hi.shape
 
+    def map(self, fn):
+        """fn applied to each present plane (it sees an e4m3 plane at its own (.., 2K) shape)."""
+        return BF2(fn(self.hi), None if self.lo is None else fn(self.lo))
+
     def view(self, *s):
-        return BF2(self.hi.view(*s), None if self.lo is None else self.lo.view(*s))
+        hi = self.hi.view(*s)
+        return BF2(hi, None if self.lo is None else self.lo.view(self._lo_shape(self.fmt, hi.shape)))
 
     def __getitem__(self, idx):
-        return BF2(self.hi[idx], None if self.lo is None else self.lo[idx])
+        if self.fmt == "f16+e4m3":      # rows only: a column cut would split the 32-column slot groups of the e4m3 plane
+            t = idx if isinstance(idx, tuple) else (idx,)
+            if len(t) >= self.hi.dim() or any(i is None or i is Ellipsis for i in t):
+                raise IndexError("BF2: fp16 + e4m3 planes can be cut along leading (row) dimensions only")
+        return self.map(lambda t: t[idx])
 
     def float(self):
         f = self.hi.float()
-        if self.lo is not None and self.lo.dtype == torch.uint8:      # fp16 + e4m3 planes of an ACTIVATION (split_f16_e4m3): [e4m3(h) | e4m3(2^10 l)]
+        if self.fmt == "f16+e4m3":      # planes of an ACTIVATION (split_f16_e4m3): [e4m3(h) | e4m3(2^10 l)]
             K = self.hi.shape[-1]
             slot1 = self.lo.view(*self.lo.shape[:-1], K // 32, 2, 32)[..., 1, :].reshape(self.hi.shape)      # slots interleaved in 32-column groups
             return f + slot1.view(torch.float8_e4m3fn).float() / 1024.0
         return f if self.lo is None else f + self.lo.float()
 
 
-def _empty_bf2(shape, device, need_lo=None):
-    need_lo = (PREC == 3) if need_lo is None else need_lo
-    hi = torch.empty(shape, dtype=torch.bfloat16, device=device)
-    lo = torch.empty(shape, dtype=torch.bfloat16, device=device) if need_lo else None
-    return BF2(hi, lo)
+def _pp(s: Optional[BF2]):
+    """(hi, lo) pointer pair of optional planes: an absent value or an absent second plane is a null pointer."""
+    return (None, None) if s is None else (_p(s.hi), _p(s.lo))
 
 
 def split(x: torch.Tensor) -> BF2:
     x = x.contiguous()
     assert x.dtype == torch.float32
-    out = _empty_bf2(x.shape, x.device)
-    _lib.check(_lib.load().hipie_split_bf16(_p(x), _p(out.hi), _p(out.lo), x.numel(), _stream()), "split_bf16")
+    out = BF2.empty(x.shape, x.device)
+    _lib.check(_lib.load().hipie_split_bf16(_p(x), *_pp(out), x.numel(), _stream()), "split_bf16")
     return out
 
 
 def split_weight(w: torch.Tensor) -> BF2:
     """Weights always carry both planes so the precision mode can be switched at run time."""
     w = w.contiguous().float()
-    out = _empty_bf2(w.shape, w.device, need_lo=True)
-    _lib.check(_lib.load().hipie_split_bf16(_p(w), _p(out.hi), _p(out.lo), w.numel(), _stream()), "split_bf16")
+    out = BF2.empty(w.shape, w.device, "bf16x2")
+    _lib.check(_lib.load().hipie_split_bf16(_p(w), *_pp(out), w.numel(), _stream()), "split_bf16")
     return out
 
 
@@ -139,10 +183,9 @@ def split_f16_e4m3(x: torch.Tensor, weight=False) -> BF2:
     x = x.contiguous().float()
     K = x.shape[-1]
     rows = x.numel() // K
-    h = torch.empty(x.shape, dtype=torch.float16, device=x.device)
-    p8 = torch.empty(x.shape[:-1] + (2 * K,), dtype=torch.uint8, device=x.device)
-    _lib.check(_lib.load().hipie_split_f16_e4m3(_p(x), _p(h), _p(p8), rows, K, 1 if weight else 0, _stream()), "split_f16_e4m3")
-    return BF2(h, p8)
+    out = BF2.empty(x.shape, x.device, "f16+e4m3")
+    _lib.check(_lib.load().hipie_split_f16_e4m3(_p(x), *_pp(out), rows, K, 1 if weight else 0, _stream()), "split_f16_e4m3")
+    return out
 
 
 def add_split(a, b=None, want_f32=False, want_split=True):
@@ -151,10 +194,24 @@ def add_split(a, b=None, want_f32=False, want_split=True):
         b = b.contiguous()
         assert a.shape == b.shape
     s = torch.empty_like(a) if want_f32 else None
-    o = _empty_bf2(a.shape, a.device) if want_split else None
-    _lib.check(_lib.load().hipie_add_split(_p(a), _p(b), _p(s), _p(o.hi) if o else None, _p(o.lo) if o else None,
-                                           a.numel(), _stream()), "add_split")
+    o = BF2.empty(a.shape, a.device) if want_split else None
+    _lib.check(_lib.load().hipie_add_split(_p(a), _p(b), _p(s), *_pp(o), a.numel(), _stream()), "add_split")
     return s, o
+
+
+_BF16, _F16 = ("bf16", "bf16x2"), ("f16", "f16x2", "f16+e4m3")       # every format whose first plane is bf16 / fp16
+# gemm precision -> (formats A may have, formats W may have, hipie_gemm_args field A's second plane feeds, field W's feeds): a second
+# plane the precision does not name is not read
+_GEMM_PLANES = {1: (_BF16, _BF16, None, None),
+                3: (("bf16x2",), ("bf16x2",), "a_lo", "w_lo"),
+                2: (_F16, _F16, None, None),
+                4: (_F16, ("f16x2",), None, "w_lo"),
+                6: (("f16+e4m3",), ("f16+e4m3",), "a8", "w8")}
+_PRODUCERS = {_BF16: "bf16 planes (split / split_weight / the default output of every kernel)",
+              ("bf16x2",): "bf16 hi + lo planes (split / split_weight / kernel outputs under set_precision(3))",
+              _F16: "fp16 planes (gemm(out_fp16=True) / layernorm(out_fp16=True) / row_softmax(out_fp16=True) / split_weight_f16)",
+              ("f16x2",): "the weight's fp16 lo plane next to its fp16 hi plane (split_weight_f16)",
+              ("f16+e4m3",): "fp16 + e4m3 planes (split_f16_e4m3 / layernorm(out_e4m3=True) / gemm(out_e4m3=True))"}
 
 
 def gemm(a: BF2, w: BF2, bias=None, act=ACT_NONE, colscale=None, residual=None, alpha=1.0, want_f32=True,
@@ -170,14 +227,12 @@ def gemm(a: BF2, w: BF2, bias=None, act=ACT_NONE, colscale=None, residual=None, 
     """
     lib = _lib.load()
     prec = PREC if prec is None else prec
-    if prec == 3 and (a.lo is None or w.lo is None):
-        raise RuntimeError("gemm: prec=3 needs lo planes")
-    if prec == 6 and not (a.lo is not None and w.lo is not None and a.lo.dtype == torch.uint8 and w.lo.dtype == torch.uint8):
-        raise RuntimeError("gemm: prec=6 takes fp16 + e4m3 planes (split_f16_e4m3 / layernorm(out_e4m3=True) / gemm(out_e4m3=True))")
-    if prec in (2, 4, 6) and not (a.hi.dtype == torch.float16 and w.hi.dtype == torch.float16):
-        raise RuntimeError("gemm: prec=2 / 4 take fp16 planes (gemm(out_fp16=True) / layernorm(out_fp16=True) / row_softmax(out_fp16=True) / split_weight_f16)")
-    if prec == 4 and (w.lo is None or w.lo.dtype != torch.float16):
-        raise RuntimeError("gemm: prec=4 (A one fp16 plane, W fp16 hi + lo) needs the weight's fp16 lo plane (split_weight_f16)")
+    if prec not in _GEMM_PLANES:
+        raise RuntimeError(f"gemm: no precision {prec} (1, 2, 3, 4 or 6)")
+    a_fmts, w_fmts, a_field, w_field = _GEMM_PLANES[prec]
+    for name, x, fmts in (("A", a, a_fmts), ("W", w, w_fmts)):
+        if x.fmt not in fmts:
+            raise RuntimeError(f"gemm: prec={prec} takes {name} as {_PRODUCERS[fmts]}, got {x.fmt} planes")
     dev = a.hi.device
     if M is None:
         assert a.hi.dim() == 2 and w.hi.dim() == 2
@@ -200,41 +255,41 @@ def gemm(a: BF2, w: BF2, bias=None, act=ACT_NONE, colscale=None, residual=None, 
     padded = transposed and batch == 1 and ldc is not None and ldc > rows_out
     ashape = (N, ldc) if padded else shape
     c_f32 = out_f32 if out_f32 is not None else (torch.empty(ashape, dtype=torch.float32, device=dev) if want_f32 else None)
-    c8 = None
-    if out_e4m3:       # fp16 plane + e4m3 planes (rows, 2N): the A operand of a following prec-6 GEMM
+    if out_e4m3:       # fp16 plane + e4m3 planes: the A operand of a following prec-6 GEMM
         assert not transposed and batch == 1 and out_split is None
-        c8 = torch.empty((rows_out, 2 * N), dtype=torch.uint8, device=dev)
-        c_split = BF2(torch.empty(ashape, dtype=torch.float16, device=dev), None)
+        c_split = BF2.empty(ashape, dev, "f16+e4m3")
         out_fp16 = True
-    elif out_fp16:     # one IEEE fp16 plane (operand of the single-pass fp16 contractions); returned as BF2(hi=fp16 tensor, lo=None)
-        c_split = out_split if out_split is not None else BF2(torch.empty(ashape, dtype=torch.float16, device=dev), None)
-        assert c_split.lo is None
+    elif out_fp16:     # one IEEE fp16 plane (operand of the single-pass fp16 contractions)
+        c_split = out_split if out_split is not None else BF2.empty(ashape, dev, "f16")
+        assert c_split.fmt == "f16"
     else:
-        c_split = out_split if out_split is not None else (_empty_bf2(ashape, dev) if want_split else None)
+        c_split = out_split if out_split is not None else (BF2.empty(ashape, dev) if want_split else None)
+    second = {a_field: a.lo, w_field: w.lo}      # hipie_gemm_args field -> the second plane it points at (key None: a plane this precision does not read)
+    if c_split is not None:
+        second["c8" if out_e4m3 else "c_lo"] = c_split.lo
+    ptr2 = lambda field: second[field].data_ptr() if second.get(field) is not None else None
+    ld2 = lambda field: second[field].stride(-2) if second.get(field) is not None else 0
     c_bits = None
     if bits_threshold is not None:       # x > threshold, bit-packed along the contiguous output dimension
         c_bits = torch.zeros((batch, N, (M + 31) // 32) if transposed else (batch, rows_out, (N + 31) // 32), dtype=torch.int32, device=dev)
     if residual is not None and ldr is None:
         ldr = residual.stride(-2) if not transposed else residual.stride(-2)
     args = _lib.GemmArgs(
-        a_hi=a.hi.data_ptr(), a_lo=a.lo.data_ptr() if (a.lo is not None and prec == 3) else None, lda=lda, a_bstride=a_bstride,
-        w_hi=w.hi.data_ptr(), w_lo=w.lo.data_ptr() if (w.lo is not None and prec in (3, 4)) else None, ldw=ldw, w_bstride=w_bstride,
+        a_hi=a.hi.data_ptr(), a_lo=ptr2("a_lo"), lda=lda, a_bstride=a_bstride,
+        w_hi=w.hi.data_ptr(), w_lo=ptr2("w_lo"), ldw=ldw, w_bstride=w_bstride,
         bias=bias.data_ptr() if bias is not None else None,
         colscale=colscale.data_ptr() if colscale is not None else None,
         residual=residual.data_ptr() if residual is not None else None,
         ldr=ldr or 0, r_bstride=r_bstride,
         c_f32=c_f32.data_ptr() if c_f32 is not None else None,
-        c_hi=c_split.hi.data_ptr() if c_split is not None else None,
-        c_lo=c_split.lo.data_ptr() if (c_split is not None and c_split.lo is not None) else None,
+        c_hi=c_split.hi.data_ptr() if c_split is not None else None, c_lo=ptr2("c_lo"),
         ldc=ldc_, c_bstride=cb,
         c_bits=c_bits.data_ptr() if c_bits is not None else None,
         bits_threshold=float(bits_threshold) if bits_threshold is not None else 0.0,
         M=M, N=N, K=K, batch=batch, act=act, prec=prec, alpha=float(alpha), transposed=1 if transposed else 0,
         c_row_map=row_map.data_ptr() if row_map is not None else None, t_row_group=t_row_group, t_row_pad=t_row_pad,
         relu_after_residual=1 if relu_after_residual else 0, c_fp16=1 if out_fp16 else 0,
-        a8=a.lo.data_ptr() if prec == 6 else None, lda8=a.lo.stride(-2) if prec == 6 else 0,
-        w8=w.lo.data_ptr() if prec == 6 else None, ldw8=w.lo.stride(-2) if prec == 6 else 0,
-        c8=c8.data_ptr() if c8 is not None else None, ldc8=2 * N if c8 is not None else 0)
+        a8=ptr2("a8"), lda8=ld2("a8"), w8=ptr2("w8"), ldw8=ld2("w8"), c8=ptr2("c8"), ldc8=ld2("c8"))
     tag = {2: "gemm_tc[f16x1]", 4: "gemm_tc[f16x2]", 6: "gemm_tc[f16+e4m3]"}.get(prec, f"gemm_tc[p{prec}]") + (":mask_embed" if c_bits is not None else "")
     if profiler.enabled and profiler.shapes:
         tag += f" {M}x{N}x{K}" + (f"x{batch}" if batch > 1 else "") + ("T" if transposed else "")
@@ -243,13 +298,11 @@ def gemm(a: BF2, w: BF2, bias=None, act=ACT_NONE, colscale=None, residual=None, 
         work = float(batch) * ((M * K + N * K) * 2.0 * (2 if prec == 3 else 1) + M * N * 4.0 + M * N / 8.0)
     with _timed(tag, work):
         _lib.check(lib.hipie_gemm(ctypes.byref(args), _stream()), "gemm")
-    if c8 is not None:
-        c_split = BF2(c_split.hi, c8)
     if padded:
         if c_f32 is not None and out_f32 is None:
             c_f32 = c_f32[:, :rows_out]
         if c_split is not None and out_split is None:
-            c_split = BF2(c_split.hi[:, :rows_out], None if c_split.lo is None else c_split.lo[:, :rows_out])
+            c_split = c_split[:, :rows_out]
     return c_f32, c_split, c_bits
 
 
@@ -280,23 +333,22 @@ def layernorm(x, gamma, beta, eps, add=None, want_f32=False, want_split=True, wa
     y = torch.empty(oshape, dtype=torch.float32, device=x.device) if want_f32 else None
     if out_e4m3:
         assert out_split is None and row_map is None
-        s = BF2(torch.empty(oshape, dtype=torch.float16, device=x.device), torch.empty(tuple(oshape[:-1]) + (2 * C,), dtype=torch.uint8, device=x.device))
+        s = BF2.empty(oshape, x.device, "f16+e4m3")
     elif out_fp16:
-        s = out_split if out_split is not None else BF2(torch.empty(oshape, dtype=torch.float16, device=x.device), None)
-        assert s.hi.dtype == torch.float16 and s.lo is None
+        s = out_split if out_split is not None else BF2.empty(oshape, x.device, "f16")
+        assert s.fmt == "f16"
     else:
-        s = out_split if out_split is not None else (_empty_bf2(oshape, x.device) if want_split else None)
+        s = out_split if out_split is not None else (BF2.empty(oshape, x.device) if want_split else None)
     ssum = torch.empty_like(x) if (want_sum and add is not None) else None
     planes = 2 if (out_e4m3 or (PREC == 3 and not out_fp16)) else 1
     nbytes = x.numel() * 4.0 * (1 + (add is not None) + (ssum is not None) + (y is not None)) + (x.numel() * 2.0 * planes if s else 0.0)
     with _timed("layernorm", nbytes):
         if out_fp16:
-            _lib.check(_lib.load().hipie_layernorm_f16(_p(x), _p(add), _p(gamma), _p(beta), float(eps), _p(ssum), _p(y), _p(s.hi),
-                                                       _p(s.lo) if out_e4m3 else None, rows, C, _p(row_map), _stream()), "layernorm_f16")
+            _lib.check(_lib.load().hipie_layernorm_f16(_p(x), _p(add), _p(gamma), _p(beta), float(eps), _p(ssum), _p(y), *_pp(s),
+                                                       rows, C, _p(row_map), _stream()), "layernorm_f16")
         else:
             _lib.check(_lib.load().hipie_layernorm(_p(x), _p(add), _p(gamma), _p(beta), float(eps), _p(ssum), _p(y),
-                                                   _p(s.hi) if s else None, _p(s.lo) if (s and s.lo is not None) else None,
-                                                   rows, C, _p(row_map), _stream()), "layernorm")
+                                                   *_pp(s), rows, C, _p(row_map), _stream()), "layernorm")
     return y, s, ssum
 
 
@@ -317,11 +369,10 @@ def groupnorm_nhwc(x, gamma, beta, eps=1e-5, groups=32, relu=False, post_add=Non
         ws = torch.empty(2 * N * groups, dtype=torch.float64, device=dev)
         _gn_ws[key] = ws
     y = out_f32 if out_f32 is not None else (torch.empty_like(x) if want_f32 else None)
-    s = _empty_bf2(x.shape, dev) if want_split else None
+    s = BF2.empty(x.shape, dev) if want_split else None
     yb = HW * C if y_bstride is None else y_bstride
     ab = HW * C if add_bstride is None else add_bstride
-    _lib.check(_lib.load().hipie_groupnorm_nhwc(_p(x), _p(gamma), _p(beta), float(eps), _p(post_add), _p(y),
-                                                _p(s.hi) if s else None, _p(s.lo) if (s and s.lo is not None) else None,
+    _lib.check(_lib.load().hipie_groupnorm_nhwc(_p(x), _p(gamma), _p(beta), float(eps), _p(post_add), _p(y), *_pp(s),
                                                 _p(ws), N, HW, C, groups, 1 if relu else 0, HW * C, yb, ab, _stream()),
                "groupnorm_nhwc")
     return y, s
@@ -331,10 +382,10 @@ def patchify(img, mean, std, P=16) -> BF2:
     B, _, H, W = img.shape
     img = img.contiguous()
     rows = B * (H // P) * (W // P)
-    out = _empty_bf2((rows, 3 * P * P), img.device)
+    out = BF2.empty((rows, 3 * P * P), img.device)
     m = (ctypes.c_float * 3)(*[float(v) for v in mean])
     s = (ctypes.c_float * 3)(*[float(v) for v in std])
-    _lib.check(_lib.load().hipie_patchify(_p(img), _p(out.hi), _p(out.lo), B, H, W, P,
+    _lib.check(_lib.load().hipie_patchify(_p(img), *_pp(out), B, H, W, P,
                                           ctypes.cast(m, ctypes.c_void_p), ctypes.cast(s, ctypes.c_void_p), _stream()),
                "patchify")
     return out
@@ -345,8 +396,8 @@ def im2col_nhwc(x, ksz=3, stride=1, pad=1) -> BF2:
     x = x.contiguous()
     Ho = (H + 2 * pad - ksz) // stride + 1
     Wo = (W + 2 * pad - ksz) // stride + 1
-    out = _empty_bf2((B * Ho * Wo, ksz * ksz * C), x.device)
-    _lib.check(_lib.load().hipie_im2col_nhwc(_p(x), _p(out.hi), _p(out.lo), B, H, W, C, ksz, stride, pad, _stream()),
+    out = BF2.empty((B * Ho * Wo, ksz * ksz * C), x.device)
+    _lib.check(_lib.load().hipie_im2col_nhwc(_p(x), *_pp(out), B, H, W, C, ksz, stride, pad, _stream()),
                "im2col_nhwc")
     return out, Ho, Wo
 
@@ -354,9 +405,8 @@ def im2col_nhwc(x, ksz=3, stride=1, pad=1) -> BF2:
 def pixel_shuffle2(g, B, H, W, C, want_f32=True, want_split=False):
     g = g.contiguous()
     y = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float32, device=g.device) if want_f32 else None
-    s = _empty_bf2((B, 2 * H, 2 * W, C), g.device) if want_split else None
-    _lib.check(_lib.load().hipie_pixel_shuffle2(_p(g), _p(y), _p(s.hi) if s else None,
-                                                _p(s.lo) if (s and s.lo is not None) else None, B, H, W, C, _stream()),
+    s = BF2.empty((B, 2 * H, 2 * W, C), g.device) if want_split else None
+    _lib.check(_lib.load().hipie_pixel_shuffle2(_p(g), _p(y), *_pp(s), B, H, W, C, _stream()),
                "pixel_shuffle2")
     return y, s
 
@@ -365,9 +415,8 @@ def maxpool2_nhwc(x, want_f32=True, want_split=False):
     B, H, W, C = x.shape
     x = x.contiguous()
     y = torch.empty((B, H // 2, W // 2, C), dtype=torch.float32, device=x.device) if want_f32 else None
-    s = _empty_bf2((B, H // 2, W // 2, C), x.device) if want_split else None
-    _lib.check(_lib.load().hipie_maxpool2_nhwc(_p(x), _p(y), _p(s.hi) if s else None,
-                                               _p(s.lo) if (s and s.lo is not None) else None, B, H, W, C, _stream()),
+    s = BF2.empty((B, H // 2, W // 2, C), x.device) if want_split else None
+    _lib.check(_lib.load().hipie_maxpool2_nhwc(_p(x), _p(y), *_pp(s), B, H, W, C, _stream()),
                "maxpool2_nhwc")
     return y, s
 
@@ -377,9 +426,8 @@ def maxpool3x3s2_nhwc(x, want_f32=True, want_split=False):
     x = x.contiguous()
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
     y = torch.empty((B, Ho, Wo, C), dtype=torch.float32, device=x.device) if want_f32 else None
-    s = _empty_bf2((B, Ho, Wo, C), x.device) if want_split else None
-    _lib.check(_lib.load().hipie_maxpool3x3s2_nhwc(_p(x), _p(y), _p(s.hi) if s else None, _p(s.lo) if (s and s.lo is not None) else None,
-                                                   B, H, W, C, _stream()), "maxpool3x3s2_nhwc")
+    s = BF2.empty((B, Ho, Wo, C), x.device) if want_split else None
+    _lib.check(_lib.load().hipie_maxpool3x3s2_nhwc(_p(x), _p(y), *_pp(s), B, H, W, C, _stream()), "maxpool3x3s2_nhwc")
     return y, s
 
 
@@ -387,16 +435,12 @@ def row_softmax(x, colbias=None, rows_per_batch=None, clampv=50000.0, sub_rowmax
     n = x.shape[-1]
     rows = x.numel() // n
     x = x.contiguous()
-    if out_fp16:
-        s = BF2(torch.empty(x.shape, dtype=torch.float16, device=x.device), None)
-    else:
-        s = _empty_bf2(x.shape, x.device) if want_split else None
+    s = BF2.empty(x.shape, x.device, "f16") if out_fp16 else (BF2.empty(x.shape, x.device) if want_split else None)
     pf = torch.empty_like(x) if want_f32 else None
     nbytes = x.numel() * 4.0 * (1 + (pf is not None)) + (x.numel() * 2.0 * (2 if (s.lo is not None) else 1) if s else 0.0)
     with _timed("row_softmax", nbytes):
         _lib.check(_lib.load().hipie_row_softmax(_p(x), _p(colbias), rows, rows_per_batch or rows, n, float(clampv),
-                                                 1 if sub_rowmax else 0, _p(s.hi) if s else None,
-                                                 _p(s.lo) if (s and s.lo is not None) else None, _p(pf), 1 if out_fp16 else 0, _stream()),
+                                                 1 if sub_rowmax else 0, *_pp(s), _p(pf), 1 if out_fp16 else 0, _stream()),
                    "row_softmax")
     return pf, s
 
@@ -408,7 +452,7 @@ def attention(q: BF2, k: BF2, v: BF2, B, H, Tq, Tk, hd, q_strides, k_strides, v_
     prec = PREC if prec is None else prec
     dev = q.hi.device
     o = torch.empty((B, Tq, H * hd), dtype=torch.float32, device=dev) if want_f32 else None
-    s = _empty_bf2((B, Tq, H * hd), dev) if want_split else None
+    s = BF2.empty((B, Tq, H * hd), dev) if want_split else None
     lo = lambda t: t.lo.data_ptr() if (t.lo is not None and prec == 3) else None
     args = _lib.AttnArgs(
         q_hi=q.hi.data_ptr(), q_lo=lo(q), k_hi=k.hi.data_ptr(), k_lo=lo(k), v_hi=v.hi.data_ptr(), v_lo=lo(v),
@@ -417,8 +461,7 @@ def attention(q: BF2, k: BF2, v: BF2, B, H, Tq, Tk, hd, q_strides, k_strides, v_
         v_bs=v_strides[0], v_ts=v_strides[1], v_hs=v_strides[2],
         rel_h=rel_h.data_ptr() if rel_h is not None else None, rel_w=rel_w.data_ptr() if rel_w is not None else None,
         kh=kh, kw=kw, key_bias=key_bias.data_ptr() if key_bias is not None else None,
-        out_f32=o.data_ptr() if o is not None else None, out_hi=s.hi.data_ptr() if s else None,
-        out_lo=s.lo.data_ptr() if (s and s.lo is not None) else None, o_bs=Tq * H * hd, o_ts=H * hd,
+        out_f32=o.data_ptr() if o is not None else None, out_hi=_pp(s)[0], out_lo=_pp(s)[1], o_bs=Tq * H * hd, o_ts=H * hd,
         B=B, H=H, Tq=Tq, Tk=Tk, hd=hd, scale=float(scale), prec=prec, key_mask=key_mask.data_ptr() if key_mask is not None else None)
     with _timed(f"attention[p{prec}]" + (":global" if Tq >= 1024 else ":small"), 4.0 * B * H * Tq * Tk * hd):
         _lib.check(_lib.load().hipie_attention(ctypes.byref(args), _stream()), "attention")
@@ -431,21 +474,20 @@ def attention_tc(q: BF2, k: BF2, vt: BF2, B, H, T, hd, q_bs, q_ts, k_bs, k_ts, s
     [80h, 80h+80) of the view); vt: BF2 (H*hd, B*T) = V transposed.  Output (B, T, H*hd)."""
     prec = PREC if prec is None else prec
     if f16:            # q / k / vt are single fp16 planes (gemm(out_fp16=True)); the output stays bf16 hi/lo for the 3-pass proj GEMM
-        assert q.hi.dtype == torch.float16 and k.hi.dtype == torch.float16 and vt.hi.dtype == torch.float16
+        assert q.fmt == k.fmt == vt.fmt == "f16"
         prec = 2
     dev = q.hi.device
     o = torch.empty((B, T, H * hd), dtype=torch.float32, device=dev) if want_f32 else None
     if out_e4m3:       # output as fp16 + e4m3 planes (the A operand of a prec-6 proj GEMM)
-        s = BF2(torch.empty((B, T, H * hd), dtype=torch.float16, device=dev), torch.empty((B, T, 2 * H * hd), dtype=torch.uint8, device=dev))
+        s = BF2.empty((B, T, H * hd), dev, "f16+e4m3")
     else:
-        s = _empty_bf2((B, T, H * hd), dev) if want_split else None
+        s = BF2.empty((B, T, H * hd), dev) if want_split else None
     lo = lambda t: _p(t.lo) if (t.lo is not None and prec == 3) else None
     fn = _lib.load().hipie_attention_tc_planes if out_e4m3 else _lib.load().hipie_attention_tc
     with _timed("attention_tc[f16x1]" if f16 else f"attention_tc[p{prec}]", 4.0 * B * H * T * T * hd):
         _lib.check(fn(
             _p(q.hi), lo(q), q_bs, q_ts, 0, H * hd, _p(k.hi), lo(k), k_bs, k_ts, 0, H * hd, _p(vt.hi), lo(vt), vt.hi.stride(0),
-            _p(rel_h), _p(rel_w), kh, kw, _p(o), _p(s.hi) if s else None, _p(s.lo) if (s and s.lo is not None) else None,
-            T * H * hd, H * hd, B, H, T, hd, float(scale), prec, _stream()), "attention_tc")
+            _p(rel_h), _p(rel_w), kh, kw, _p(o), *_pp(s), T * H * hd, H * hd, B, H, T, hd, float(scale), prec, _stream()), "attention_tc")
     return o, s
 
 
@@ -484,7 +526,7 @@ def relpos_bias_tc_f16(q_f16: torch.Tensor, q_strides, table: BF2, axis, qh, qw,
     ksize = table.hi.shape[1]
     rel = torch.empty((B, H, qh * qw, ksize), dtype=torch.float32, device=q_f16.device)
     with _timed("relpos_bias_tc"):
-        _lib.check(_lib.load().hipie_relpos_bias_tc_f16(_p(q_f16), q_strides[0], q_strides[1], q_strides[2], _p(table.hi), _p(table.lo), axis,
+        _lib.check(_lib.load().hipie_relpos_bias_tc_f16(_p(q_f16), q_strides[0], q_strides[1], q_strides[2], *_pp(table), axis,
                                                         qh, qw, ksize, _p(rel), B, H, hd, _stream()), "relpos_bias_tc_f16")
     return rel
 
@@ -518,7 +560,7 @@ def msda_fused(value, spatial_shapes, level_start_index, offs_logits, reference_
     vdt = 2 if value.dtype == torch.bfloat16 else (3 if value.dtype == torch.float16 else 0)
     dev = value.device
     if want_split:
-        s = _empty_bf2((N, Lq, M * D), dev)
+        s = BF2.empty((N, Lq, M * D), dev)
         out, out_lo = s.hi, s.lo
     else:
         s = None
@@ -605,9 +647,8 @@ def sine_embed(pos, want_f32=False, want_split=True):
     if pos.dim() > 2:
         assert pos.stride(-3) == ld * pos.shape[-2], "sine_embed: rows must be uniformly strided"
     out = torch.empty((rows, 512), dtype=torch.float32, device=pos.device) if want_f32 else None
-    s = _empty_bf2((rows, 512), pos.device) if want_split else None
-    _lib.check(_lib.load().hipie_sine_embed(_p(pos), ld, rows, _p(out), _p(s.hi) if s else None,
-                                            _p(s.lo) if (s and s.lo is not None) else None, _stream()), "sine_embed")
+    s = BF2.empty((rows, 512), pos.device) if want_split else None
+    _lib.check(_lib.load().hipie_sine_embed(_p(pos), ld, rows, _p(out), *_pp(s), _stream()), "sine_embed")
     return out, s
 
 
@@ -673,12 +714,11 @@ def clip_patches(image01, S, P, mean, std):
     _, H, W = image01.shape
     G, K = S // P, 3 * P * P
     ld = (K + 7) // 8 * 8
-    out = BF2(torch.zeros((G * G, ld), dtype=torch.bfloat16, device=image01.device),
-              torch.zeros((G * G, ld), dtype=torch.bfloat16, device=image01.device) if PREC == 3 else None)
+    out = BF2.zeros((G * G, ld), image01.device)
     m3, s3 = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
     with _timed("clip_patches"):
         _lib.check(_lib.load().hipie_clip_patches(_p(image01), H, W, S, P, ctypes.cast(m3, ctypes.c_void_p), ctypes.cast(s3, ctypes.c_void_p),
-                                                  _p(out.hi), _p(out.lo) if out.lo is not None else None, ld, _stream()), "clip_patches")
+                                                  *_pp(out), ld, _stream()), "clip_patches")
     return out
 
 
@@ -704,11 +744,11 @@ def sam_attention(q, k, v, B, H, Tq, Tk, hd, q_bs, q_ld, kv_bs, kv_ld, q_index=N
     batch to its q / kv batch.  Returns (out_f32 (B, Tq, H*hd) or None, BF2 planes or None)."""
     dev = q.device
     o = torch.empty((B, Tq, H * hd), dtype=torch.float32, device=dev) if want_f32 else None
-    s = _empty_bf2((B, Tq, H * hd), dev) if want_split else None
+    s = BF2.empty((B, Tq, H * hd), dev) if want_split else None
     tag = "sam_attention:" + ("fewq" if Tq <= 8 else "fewk")
     with _timed(tag, 4.0 * B * H * Tq * Tk * hd):
         _lib.check(_lib.load().hipie_sam_attention(_p(q), q_bs, q_ld, _p(q_index), _p(k), _p(v), kv_bs, kv_ld, _p(kv_index), _p(o),
-                                                   _p(s.hi) if s else None, _p(s.lo) if (s and s.lo is not None) else None, Tq * H * hd, H * hd,
+                                                   *_pp(s), Tq * H * hd, H * hd,
                                                    B, H, Tq, Tk, hd, float(hd ** -0.5), _stream()), "sam_attention")
     return o, s
 
