@@ -714,44 +714,102 @@ class Engine:
         new_l, _, _ = ops.gemm(out_l, wol, bias=bol, colscale=W[p + ".gamma_l"], residual=l)
         return new_v.view(B, S, 256), new_v_s.view(B, S, 256), new_l.view(B, Lt, Ld)
 
-    # ------------------------------------------------------------ DETR: input projections + transformer + heads
-    def detr_inputs(self, feats, pad_mask, B, any_pad=True):
-        """input_proj + sine positions + flatten (H/models/ddetrs_dn.py:821-847, deformable_transformer_dino.py:187-207).
-        feats: {res3,res4,res5: (fp32 NHWC, BF2)}; pad_mask (B, H, W) bool.  -> dict"""
-        W = self.W
-        dd = "detr.detr"
+    # ------------------------------------------------------------ deformable-DINO stages of the DETR and MaskDINO branches
+    def _levels(self, feats):
+        """The four encoder levels (res3..res5 and the 3x3 stride-2 level on res5) -> (lv, shapes, starts, S, shapes_t, lsi_t)"""
         lv = [feats["res3"], feats["res4"], feats["res5"]]
         shapes = [tuple(f[0].shape[1:3]) for f in lv]
         h5, w5 = shapes[2]
         shapes.append(((h5 + 2 - 3) // 2 + 1, (w5 + 2 - 3) // 2 + 1))
-        S = sum(h * w for h, w in shapes)
-        src = torch.empty(B, S, 256, device=self.device)
+        return (lv, shapes) + self._level_index(shapes)
+
+    def _level_index(self, shapes):
+        """Levels flattened in the order of `shapes` -> (starts, S, shapes_t, lsi_t), the last two as device constants."""
         starts = [0]
         for h, w in shapes[:-1]:
             starts.append(starts[-1] + h * w)
-        masks, poses = [], []
+        S = starts[-1] + shapes[-1][0] * shapes[-1][1]
+        return starts, S, self._dev_const([list(x) for x in shapes], torch.long), self._dev_const(list(starts), torch.long)
+
+    def _input_proj(self, prefix, lv, starts, S, B):
+        """input_proj.{0,1,2} (1x1 conv + GN on res3..res5) and input_proj.3 (3x3/2 conv + GN on res5), written level-flattened into
+        one (B, S, 256) buffer (H/models/ddetrs_dn.py:821-847; maskdino_encoder.py:380-396)."""
+        W = self.W
+        src = torch.empty(B, S, 256, device=self.device)
         for l in range(3):
-            self.conv1x1_gn(lv[l][1], f"{dd}.input_proj.{l}.0", f"{dd}.input_proj.{l}.1", out_view=src[:, starts[l]:], y_bstride=S * 256)
-            m = F.interpolate(pad_mask[None].float(), size=shapes[l]).to(torch.bool)[0]
-            masks.append(m)
+            self.conv1x1_gn(lv[l][1], f"{prefix}.input_proj.{l}.0", f"{prefix}.input_proj.{l}.1", out_view=src[:, starts[l]:], y_bstride=S * 256)
         cols, Ho, Wo = ops.im2col_nhwc(lv[2][0], 3, 2, 1)
-        wk, bk = W.conv_kxk(f"{dd}.input_proj.3.0")
+        wk, bk = W.conv_kxk(f"{prefix}.input_proj.3.0")
         y, _, _ = ops.gemm(cols, wk, bias=bk)
-        ops.groupnorm_nhwc(y.view(B, Ho * Wo, 256), W[f"{dd}.input_proj.3.1.weight"], W[f"{dd}.input_proj.3.1.bias"],
+        ops.groupnorm_nhwc(y.view(B, Ho * Wo, 256), W[f"{prefix}.input_proj.3.1.weight"], W[f"{prefix}.input_proj.3.1.bias"],
                            out_f32=src[:, starts[3]:], y_bstride=S * 256)
+        return src
+
+    @staticmethod
+    def _level_pos(masks, offset, level_embed):
+        """Per-level sine position + level_embed, level-flattened -> (B, S, 256) (deformable_transformer_dino.py:187-207;
+        maskdino_encoder.py:94-101)."""
+        return torch.cat([_sine_pos(m, 128, offset) + level_embed[l].view(1, 1, -1) for l, m in enumerate(masks)], 1).contiguous()
+
+    def _enc_proposals(self, prefix, memory, shapes, mask_flat, B, S, pad_fill):
+        """Two-stage encoder output (deformable_transformer_dino.py:222-224; maskdino_decoder.py:413-415): enc_output + LN on the memory,
+        invalid proposals (and with `pad_fill` padded pixels) zeroed -> (unsigmoided proposals (B, S, 4), om_n (B*S, 256), om_ns)"""
+        W = self.W
+        props, valid = self.proposals(shapes, mask_flat, B, self.device)
+        om = memory.masked_fill(mask_flat.unsqueeze(-1), 0.0) if pad_fill else memory
+        om = om.masked_fill(~valid, 0.0)
+        _, om_s = ops.add_split(om.view(B * S, 256))
+        we, be = W.lin(prefix + ".enc_output")
+        y, _, _ = ops.gemm(om_s, we, bias=be)
+        om_n, om_ns, _ = ops.layernorm(y, W[prefix + ".enc_output_norm.weight"], W[prefix + ".enc_output_norm.bias"], 1e-5,
+                                       want_f32=True, want_split=True)
+        return props, om_n, om_ns
+
+    def _select_queries(self, om_n, props, scores, nq, bbox_prefix, B, forced_topk):
+        """Two-stage selection (deformable_transformer_dino.py:225-230; maskdino_decoder.py:416-426): top-k of `scores` (B, S), the
+        selected encoder outputs and their boxes sigmoid(bbox MLP + proposal).  -> (topk, sel (B, nq, 256), sel_s, ref (B, nq, 4))"""
+        # on the device (ops.topk: values descending, lowest index first among exact ties -> deterministic)
+        topk = ops.topk(scores.contiguous(), nq)[1].long() if forced_topk is None else forced_topk
+        # the bbox MLP only on the selected rows (same values as computing all and gathering)
+        sel = torch.gather(om_n.view(B, -1, 256), 1, topk.unsqueeze(-1).expand(-1, -1, 256)).contiguous()
+        _, sel_s = ops.add_split(sel)
+        delta = self.mlp(sel_s.view(B * nq, 256), bbox_prefix, 3).view(B, nq, 4)
+        ref = (delta + torch.gather(props, 1, topk.unsqueeze(-1).expand(-1, -1, 4))).sigmoid()
+        return topk, sel, sel_s, ref
+
+    def _dino_decoder(self, prefix, bbox_prefixes, tgt, tgt_s, ref, vr2, memory_s, mask_flat, shapes_t, lsi_t, B, Q, S):
+        """Decoder loop (deformable_transformer_dino.py:467-525; dino_decoder.py:94-168), one layer per box MLP in `bbox_prefixes`;
+        vr2 (B, L, 4) valid ratios.  -> (hs: [(tgt, tgt_s)] per layer, refs: the box refined by each layer)"""
+        hs, refs = [], []
+        for lid, bbox_prefix in enumerate(bbox_prefixes):
+            ref_in = (ref[:, :, None] * vr2[:, None]).contiguous()              # (B, Q, L, 4)
+            _, sine_s = ops.sine_embed(ref_in[:, :, 0, :])                      # (B*Q, 512) planes, one kernel
+            qpos = self.mlp(sine_s, prefix + ".ref_point_head", 2).view(B, Q, 256)
+            tgt, tgt_s = self.decoder_layer(f"{prefix}.layers.{lid}", tgt, tgt_s, qpos, ref_in, memory_s, mask_flat, shapes_t, lsi_t, B, Q, S)
+            tmp = self.mlp(tgt_s.view(B * Q, 256), bbox_prefix, 3).view(B, Q, 4)
+            ref = (tmp + inverse_sigmoid(ref)).sigmoid()
+            hs.append((tgt, tgt_s))
+            refs.append(ref)
+        return hs, refs
+
+    # ------------------------------------------------------------ DETR: input projections + transformer + heads
+    def detr_inputs(self, feats, pad_mask, B, any_pad=True):
+        """input_proj + sine positions + flatten (H/models/ddetrs_dn.py:821-847, deformable_transformer_dino.py:187-207).
+        feats: {res3,res4,res5: (fp32 NHWC, BF2)}; pad_mask (B, H, W) bool.  -> dict"""
+        dd = "detr.detr"
+        lv, shapes, starts, S, shapes_t, lsi_t = self._levels(feats)
+        src = self._input_proj(dd, lv, starts, S, B)
+        masks = [F.interpolate(pad_mask[None].float(), size=shapes[l]).to(torch.bool)[0] for l in range(3)]
         masks.append(F.interpolate(masks[0][None].float(), size=shapes[3]).to(torch.bool)[0])
-        lvl_embed = W[f"{dd}.transformer.level_embed"]
-        make_pos = lambda: torch.cat([_sine_pos(masks[l], 128, -0.5) + lvl_embed[l].view(1, 1, -1) for l in range(4)], 1).contiguous()
+        make_pos = lambda: self._level_pos(masks, -0.5, self.W[f"{dd}.transformer.level_embed"])
         # without padding the masks are all-False and the encoding depends on the shapes only: computed once per resolution
-        pos = make_pos() if any_pad else W.cached(("sine_pos_detr", B, tuple(shapes)), make_pos)
+        pos = make_pos() if any_pad else self.W.cached(("sine_pos_detr", B, tuple(shapes)), make_pos)
         mask_flat = torch.cat([m.flatten(1) for m in masks], 1)
         vr = []
         for m in masks:
             _, Hh, Ww = m.shape
             vr.append(torch.stack([torch.sum(~m[:, 0, :], 1).float() / Ww, torch.sum(~m[:, :, 0], 1).float() / Hh], -1))
         valid_ratios = torch.stack(vr, 1)
-        shapes_t = self._dev_const([list(x) for x in shapes], torch.long)
-        lsi_t = self._dev_const(list(starts), torch.long)
         return dict(src=src, pos=pos, mask_flat=mask_flat, any_pad=any_pad, valid_ratios=valid_ratios,
                     shapes=shapes, shapes_t=shapes_t, lsi_t=lsi_t, S=S, starts=starts)
 
@@ -768,41 +826,21 @@ class Engine:
         for i in range(hp.get("enc_layers", 6)):
             src, src_s = self.encoder_layer(f"{t}.encoder.layers.{i}", src, src_s, pos, ref_enc, mask_flat, shapes_t, lsi_t, B, S, shapes_host=shapes)
         memory, memory_s = src, src_s
-        # two-stage proposals (:222-230): enc_output + LN on masked memory, Still_Classifier score, top-k
-        props, valid = self.proposals(shapes, di["mask_flat"], B, self.device)
-        om = memory.masked_fill(di["mask_flat"].unsqueeze(-1), 0.0).masked_fill(~valid, 0.0)
-        _, om_s = ops.add_split(om.view(B * S, 256))
-        we, be = W.lin(t + ".enc_output")
-        y, _, _ = ops.gemm(om_s, we, bias=be)
-        om_n, om_ns, _ = ops.layernorm(y, W[t + ".enc_output_norm.weight"], W[t + ".enc_output_norm.bias"], 1e-5, want_f32=True, want_split=True)
+        # two-stage proposals: enc_output + LN on the masked memory, Still_Classifier score, top-k, bbox_embed[nd]
+        props, om_n, om_ns = self._enc_proposals(t, memory, shapes, di["mask_flat"], B, S, pad_fill=True)
         nd = hp.get("dec_layers", 6)
         wc, bc = W.lin(f"detr.detr.class_embed.{nd}.body")
         scores, _, _ = ops.gemm(om_ns, wc, bias=bc)
         scores = scores.view(B, S)
         nq = hp.get("num_queries", 900)
-        # two-stage selection on the device (ops.topk: values descending, lowest index first among exact ties -> deterministic)
-        topk = ops.topk(scores.contiguous(), nq)[1].long() if forced_topk is None else forced_topk
-        # bbox_embed[nd] only on the selected rows (same values as computing all and gathering, :226-229)
-        sel = torch.gather(om_n.view(B, S, 256), 1, topk.unsqueeze(-1).expand(-1, -1, 256)).reshape(B * nq, 256).contiguous()
-        _, sel_s = ops.add_split(sel)
-        delta = self.mlp(sel_s, f"detr.detr.bbox_embed.{nd}", 3).view(B, nq, 4)
-        ref = (delta + torch.gather(props, 1, topk.unsqueeze(-1).expand(-1, -1, 4))).sigmoid()
+        topk, _, _, ref = self._select_queries(om_n, props, scores, nq, f"detr.detr.bbox_embed.{nd}", B, forced_topk)
         nbg = hp.get("num_bg", 10)
         tgt = torch.cat([W[t + ".tgt_embed_bg.weight"], W[t + ".tgt_embed.weight"]], 0)[None].repeat(B, 1, 1).contiguous()
         ref = torch.cat([W[t + ".bg_query_refs.weight"][None].repeat(B, 1, 1), ref], 1).contiguous()
-        Q = nbg + nq
         _, tgt_s = ops.add_split(tgt)
         vr2 = torch.cat([di["valid_ratios"], di["valid_ratios"]], -1)           # (B, L, 4)
-        hs, refs = [], []
-        for lid in range(nd):
-            ref_in = (ref[:, :, None] * vr2[:, None]).contiguous()              # (B, Q, L, 4)
-            _, sine_s = ops.sine_embed(ref_in[:, :, 0, :])                      # (B*Q, 512) planes, one kernel
-            qpos = self.mlp(sine_s, t + ".decoder.ref_point_head", 2).view(B, Q, 256)
-            tgt, tgt_s = self.decoder_layer(f"{t}.decoder.layers.{lid}", tgt, tgt_s, qpos, ref_in, memory_s, mask_flat, shapes_t, lsi_t, B, Q, S)
-            tmp = self.mlp(tgt_s.view(B * Q, 256), f"detr.detr.bbox_embed.{lid}", 3).view(B, Q, 4)
-            ref = (tmp + inverse_sigmoid(ref)).sigmoid()
-            hs.append((tgt, tgt_s))
-            refs.append(ref)
+        hs, refs = self._dino_decoder(t + ".decoder", [f"detr.detr.bbox_embed.{lid}" for lid in range(nd)], tgt, tgt_s, ref, vr2,
+                                      memory_s, mask_flat, shapes_t, lsi_t, B, nbg + nq, S)
         return dict(hs=hs, refs=refs, memory=memory, memory_s=memory_s, lang_hidden=lang_hidden, enc_scores=scores, topk=topk)
 
     def vl_align(self, prefix, q_s, lang_hidden, B, Q):
@@ -860,31 +898,12 @@ class Engine:
         transformer_decoder/maskdino_decoder.py:377-529, dino_decoder.py:94-168)."""
         W, hp = self.W, self.hp
         pd, pr = "detr.mask_dino.pixel_decoder", "detr.mask_dino.predictor"
-        lv = [feats["res3"], feats["res4"], feats["res5"]]
-        shapes = [tuple(f[0].shape[1:3]) for f in lv]
-        h5, w5 = shapes[2]
-        shapes.append(((h5 + 2 - 3) // 2 + 1, (w5 + 2 - 3) // 2 + 1))
-        S = sum(h * w for h, w in shapes)
-        starts = [0]
-        for h, w in shapes[:-1]:
-            starts.append(starts[-1] + h * w)
-        src = torch.empty(B, S, 256, device=self.device)
-        for l in range(3):
-            self.conv1x1_gn(lv[l][1], f"{pd}.input_proj.{l}.0", f"{pd}.input_proj.{l}.1", out_view=src[:, starts[l]:], y_bstride=S * 256)
-        cols, Ho, Wo = ops.im2col_nhwc(lv[2][0], 3, 2, 1)
-        wk, bk = W.conv_kxk(f"{pd}.input_proj.3.0")
-        y, _, _ = ops.gemm(cols, wk, bias=bk)
-        ops.groupnorm_nhwc(y.view(B, Ho * Wo, 256), W[f"{pd}.input_proj.3.1.weight"], W[f"{pd}.input_proj.3.1.bias"],
-                           out_f32=src[:, starts[3]:], y_bstride=S * 256)
-        lvl_embed = W[pd + ".transformer.level_embed"]
-        def make_pos_md():      # MaskDINO always passes mask=None (maskdino_encoder.py:82-88): shape-only, cached per resolution
-            zeros = [torch.zeros(B, h, w, dtype=torch.bool, device=self.device) for h, w in shapes]
-            return torch.cat([_sine_pos(zeros[l], 128, 0.0) + lvl_embed[l].view(1, 1, -1) for l in range(4)], 1).contiguous()
-        pos = W.cached(("sine_pos_md", B, tuple(shapes)), make_pos_md)
-        ones_vr = torch.ones(B, 4, 2, device=self.device)
-        ref_enc = self.encoder_reference_points(shapes, ones_vr, self.device)
-        shapes_t = self._dev_const([list(x) for x in shapes], torch.long)
-        lsi_t = self._dev_const(list(starts), torch.long)
+        lv, shapes, starts, S, shapes_t, lsi_t = self._levels(feats)
+        src = self._input_proj(pd, lv, starts, S, B)
+        # MaskDINO always passes mask=None (maskdino_encoder.py:82-88): shape-only, cached per resolution
+        pos = W.cached(("sine_pos_md", B, tuple(shapes)), lambda: self._level_pos(
+            [torch.zeros(B, h, w, dtype=torch.bool, device=self.device) for h, w in shapes], 0.0, W[pd + ".transformer.level_embed"]))
+        ref_enc = self.encoder_reference_points(shapes, torch.ones(B, 4, 2, device=self.device), self.device)
         _, src_s = ops.add_split(src)
         for i in range(hp.get("md_enc_layers", 6)):
             src, src_s = self.encoder_layer(f"{pd}.transformer.encoder.layers.{i}", src, src_s, pos, ref_enc, None, shapes_t, lsi_t, B, S,
@@ -914,44 +933,22 @@ class Engine:
         # ---- decoder: levels re-flattened coarse -> fine (maskdino_decoder.py:398-404)
         order = [3, 2, 1, 0]
         dshapes = [shapes[i] for i in order]
-        dstarts = [0]
-        for h, w in dshapes[:-1]:
-            dstarts.append(dstarts[-1] + h * w)
         mem = torch.cat([src[:, starts[i]:starts[i] + shapes[i][0] * shapes[i][1]] for i in order], 1).contiguous()
         _, mem_s = ops.add_split(mem)
-        dshapes_t = self._dev_const([list(x) for x in dshapes], torch.long)
-        dlsi_t = self._dev_const(list(dstarts), torch.long)
+        _, _, dshapes_t, dlsi_t = self._level_index(dshapes)
         zmask = torch.zeros(B, S, dtype=torch.bool, device=self.device)
-        props, valid = self.proposals(dshapes, zmask, B, self.device)
-        om = mem.masked_fill(~valid, 0.0)
-        _, om_s = ops.add_split(om.view(B * S, 256))
-        we, be = W.lin(pr + ".enc_output")
-        y, _, _ = ops.gemm(om_s, we, bias=be)
-        om_n, om_ns, _ = ops.layernorm(y, W[pr + ".enc_output_norm.weight"], W[pr + ".enc_output_norm.bias"], 1e-5, want_f32=True, want_split=True)
+        props, om_n, om_ns = self._enc_proposals(pr, mem, dshapes, zmask, B, S, pad_fill=False)
         wc, bc = W.lin(pr + ".class_embed")
         cls_all, _, _ = ops.gemm(om_ns, wc, bias=bc)
         enc_scores = cls_all.view(B, S, -1).max(-1)[0]
         nq = hp.get("md_queries", 300)
-        topk = ops.topk(enc_scores.contiguous(), nq)[1].long() if forced_topk is None else forced_topk
-        tgt = torch.gather(om_n.view(B, S, 256), 1, topk.unsqueeze(-1).expand(-1, -1, 256)).contiguous()
-        _, tgt_s = ops.add_split(tgt)
-        delta = self.mlp(tgt_s.view(B * nq, 256), pr + "._bbox_embed", 3).view(B, nq, 4)
-        ref = (delta + torch.gather(props, 1, topk.unsqueeze(-1).expand(-1, -1, 4))).sigmoid()
-        vr2 = torch.ones(B, 4, 4, device=self.device)
-        refs = [ref]
-        hs_last = None
-        nl = hp.get("md_dec_layers", 9)
-        for lid in range(nl):
-            ref_in = (ref[:, :, None] * vr2[:, None]).contiguous()
-            _, sine_s = ops.sine_embed(ref_in[:, :, 0, :])                      # (B*Q, 512) planes, one kernel
-            qpos = self.mlp(sine_s, pr + ".decoder.ref_point_head", 2).view(B, nq, 256)
-            tgt, tgt_s = self.decoder_layer(f"{pr}.decoder.layers.{lid}", tgt, tgt_s, qpos, ref_in, mem_s, None, dshapes_t, dlsi_t, B, nq, S)
-            tmp = self.mlp(tgt_s.view(B * nq, 256), pr + "._bbox_embed", 3).view(B, nq, 4)
-            ref = (tmp + inverse_sigmoid(ref)).sigmoid()
-            refs.append(ref)
+        topk, tgt, tgt_s, ref = self._select_queries(om_n, props, enc_scores, nq, pr + "._bbox_embed", B, forced_topk)
+        dec_hs, refs = self._dino_decoder(pr + ".decoder", [pr + "._bbox_embed"] * hp.get("md_dec_layers", 9), tgt, tgt_s, ref,
+                                          torch.ones(B, 4, 4, device=self.device), mem_s, None, dshapes_t, dlsi_t, B, nq, S)
+        refs = [ref] + refs
         # intermediate = decoder_norm(output); prediction heads apply decoder_norm again (double LN, dino_decoder.py:163 + :521)
         gn, bn = W[pr + ".decoder_norm.weight"], W[pr + ".decoder_norm.bias"]
-        hs, hs_s, _ = ops.layernorm(tgt.view(B * nq, 256), gn, bn, 1e-5, want_f32=True, want_split=True)
+        hs, hs_s, _ = ops.layernorm(dec_hs[-1][0].view(B * nq, 256), gn, bn, 1e-5, want_f32=True, want_split=True)
         dec, dec_s, _ = ops.layernorm(hs, gn, bn, 1e-5, want_f32=True, want_split=True)
         cls_emb, cls_emb_s, _ = ops.gemm(dec_s, wc, bias=bc, want_split=True)                              # (B*nq, 256) "pred_logits" embedding
         me_s = self.mlp(dec_s, pr + ".mask_embed", 3, last_f32=False)                                      # BF2 (B*nq, 256)

@@ -58,6 +58,30 @@ class Spec:
         self.add(p + ".in_proj_bias", (3 * d,), "b")
         self.linear(p + ".out_proj", d, d)
 
+    def input_proj(self, p, d, ch):
+        """1x1 conv + GN on each of the three backbone levels, then the 3x3 stride-2 conv + GN on the last."""
+        for l in range(3):
+            self.conv(f"{p}.input_proj.{l}.0", d, ch[l], 1)
+            self.norm(f"{p}.input_proj.{l}.1", d)
+        self.conv(f"{p}.input_proj.3.0", d, ch[2], 3)
+        self.norm(f"{p}.input_proj.3.1", d)
+
+    def deformable_encoder_layer(self, p, d, ff):
+        self.msda(p + ".self_attn", d)
+        self.norm(p + ".norm1", d)
+        self.linear(p + ".linear1", ff, d)
+        self.linear(p + ".linear2", d, ff)
+        self.norm(p + ".norm2", d)
+
+    def deformable_decoder_layer(self, p, d, ff):
+        self.msda(p + ".cross_attn", d)
+        self.norm(p + ".norm1", d)
+        self.mha(p + ".self_attn", d)
+        self.norm(p + ".norm2", d)
+        self.linear(p + ".linear1", ff, d)
+        self.linear(p + ".linear2", d, ff)
+        self.norm(p + ".norm3", d)
+
 
 def backbone_channels(hp):
     if hp["backbone"] == "vit":
@@ -113,11 +137,7 @@ def build_spec(hp) -> Spec:
             cout *= 2
     ch = backbone_channels(hp)
     dd = "detr.detr"
-    for l in range(3):
-        s.conv(f"{dd}.input_proj.{l}.0", d, ch[l], 1)
-        s.norm(f"{dd}.input_proj.{l}.1", d)
-    s.conv(f"{dd}.input_proj.3.0", d, ch[2], 3)
-    s.norm(f"{dd}.input_proj.3.1", d)
+    s.input_proj(dd, d, ch)
     t = dd + ".transformer"
     s.add(t + ".level_embed", (4, d), "normal1")
     vl = t + ".encoder.vl_layers.0.b_attn"
@@ -130,21 +150,9 @@ def build_spec(hp) -> Spec:
                       "out_v_proj": (d, E), "out_l_proj": (lang, E)}.items():
         s.linear(f"{vl}.attn.{n}", o, i)
     for i in range(hp.get("enc_layers", 6)):
-        p = f"{t}.encoder.layers.{i}"
-        s.msda(p + ".self_attn", d)
-        s.norm(p + ".norm1", d)
-        s.linear(p + ".linear1", ff, d)
-        s.linear(p + ".linear2", d, ff)
-        s.norm(p + ".norm2", d)
+        s.deformable_encoder_layer(f"{t}.encoder.layers.{i}", d, ff)
     for i in range(hp.get("dec_layers", 6)):
-        p = f"{t}.decoder.layers.{i}"
-        s.msda(p + ".cross_attn", d)
-        s.norm(p + ".norm1", d)
-        s.mha(p + ".self_attn", d)
-        s.norm(p + ".norm2", d)
-        s.linear(p + ".linear1", ff, d)
-        s.linear(p + ".linear2", d, ff)
-        s.norm(p + ".norm3", d)
+        s.deformable_decoder_layer(f"{t}.decoder.layers.{i}", d, ff)
     s.mlp(t + ".decoder.ref_point_head", [2 * d, d, d])
     s.add(t + ".tgt_embed.weight", (hp.get("num_queries", 900), d), "normal1")
     s.add(t + ".tgt_embed_bg.weight", (hp.get("num_bg", 10), d), "normal1")
@@ -173,19 +181,10 @@ def build_spec(hp) -> Spec:
     # ---- MaskDINO branch
     pd = "detr.mask_dino.pixel_decoder"
     mff = hp.get("md_dim_ff", 2048)
-    for l in range(3):
-        s.conv(f"{pd}.input_proj.{l}.0", d, ch[l], 1)
-        s.norm(f"{pd}.input_proj.{l}.1", d)
-    s.conv(f"{pd}.input_proj.3.0", d, max(ch), 3)
-    s.norm(f"{pd}.input_proj.3.1", d)
+    s.input_proj(pd, d, ch)
     for i in range(hp.get("md_enc_layers", 6)):
-        p = f"{pd}.transformer.encoder.layers.{i}"
-        s.msda(p + ".self_attn", d)
-        s.norm(p + ".norm1", d)
-        s.linear(p + ".linear1", mff, d)
-        s.linear(p + ".linear2", d, mff)
-        s.norm(p + ".norm2", d)
-    s.add(pd + ".transformer.level_embed", (4, d), "normal1")
+        s.deformable_encoder_layer(f"{pd}.transformer.encoder.layers.{i}", d, mff)
+    s.add(pd + ".transformer.level_embed", (4, d), "normal1")       # after the encoder layers, unlike DETR's
     s.add(pd + ".mask_features.0.weight", (d, d, 2, 2))
     s.add(pd + ".mask_features.0.bias", (d,), "b")
     s.norm(pd + ".mask_features.1", d)
@@ -203,14 +202,7 @@ def build_spec(hp) -> Spec:
     s.mlp(pr + ".mask_embed", [d, d, d, d])
     s.norm(pr + ".decoder_norm", d)
     for i in range(hp.get("md_dec_layers", 9)):
-        p = f"{pr}.decoder.layers.{i}"
-        s.msda(p + ".cross_attn", d)
-        s.norm(p + ".norm1", d)
-        s.mha(p + ".self_attn", d)
-        s.norm(p + ".norm2", d)
-        s.linear(p + ".linear1", mff, d)
-        s.linear(p + ".linear2", d, mff)
-        s.norm(p + ".norm3", d)
+        s.deformable_decoder_layer(f"{pr}.decoder.layers.{i}", d, mff)
     s.mlp(pr + ".decoder.ref_point_head", [2 * d, d, d])
     s.mlp(pr + "._bbox_embed", [d, d, d, 4])
     for i in range(hp.get("md_dec_layers", 9) + 2):
