@@ -2,7 +2,8 @@
 
 The device kernels (csrc/common.cuh: split4_f16_e4m3, e4m3_slot0; csrc/gemm_tc.cu prec 6) are checked against these formulas in
 tests/test_kernels_gpu.py; here the formulas themselves are pinned: the layout of the e4m3 planes, the reconstruction the host
-helper BF2.float() performs, and the accuracy class of the fp16 + e4m3 split product against an fp64 product."""
+helper BF2.float() performs, the accuracy class of the fp16 + e4m3 split product against an fp64 product, and the operand range that
+class holds in (tests/test_precision_range_gpu.py asserts the same range on the device, on the same operands)."""
 import math
 
 import pytest
@@ -57,6 +58,98 @@ def test_split_product_accuracy_class(K):
     err_split, err_one, err_x3 = (split - exact).abs().max().item(), (one_pass - exact).abs().max().item(), (bf16x3 - exact).abs().max().item()
     assert err_split < 6e-5 * math.sqrt(K) * 1.5 * 0.05 * 4
     assert err_split < err_one / 8 and err_split < 4 * err_x3 + 1e-7, (err_split, err_one, err_x3)
+
+
+# ---------------------------------------------------------------------------------------------------- the range of the split
+# Per product a.w the split drops nothing but Al.Wl (2^-22 |a w|) and rounds the four factors of the two cross terms (each
+# <= 2^-11 |a w|) to e4m3, 2^-4 relative at most while they are normal: <= 2^-13 |a w| in the worst case, ~2^-15.5 rms.  Over K
+# products with independent errors the sum then carries ~2^-15.5 sqrt(sum p^2) / sum |p| of sum |p|, i.e. 2^-20 at K = 1280 for
+# unit-spread operands; max |C - A.W| / (|A|.|W|^T) over a 64 x 48 output comes out at 2^-19 (one fp16 pass: 2^-14.3).  The
+# lower end of the range is gradual: RANGE_BOUND is met down to activation rows of max 2^-4 (2^-17.4 there).  Rows dominated by a
+# few in-range outlier channels average over fewer products (2^-16.8 with 8 channels at 300) and are held at OUTLIER_BOUND.
+#
+# The range ends where a factor leaves e4m3's normal range:
+#   slot 0 of an activation, e4m3(Ah), saturates at 448 (464 rounds down to it): past that the Ah.Wl term is lost in proportion;
+#   slot 1 of an activation, e4m3(2^10 Al) <= 2^-1 |a|, turns subnormal for rows below ~2^-5 and vanishes below ~2^-9;
+#   slot 1 of a weight, e4m3(2^4 Wh), saturates at |W| = 28; slot 0, e4m3(2^14 Wl) <= 2^3 |w|, turns subnormal for rows below ~2^-9.
+# Outside it the split is still a correction of the fp16 pass: finite and no worse than the fp16 pass alone.
+RANGE_BOUND, OUTLIER_BOUND = 2.0 ** -17, 2.0 ** -16
+
+
+def range_case(kind, value, K=1280, rows=64, cols=48, seed=0):
+    """(A, W) fp32 operands of one point of the range: kind "rowmax" (every activation row scaled to max |a| = value), "outliers"
+    (8 activation channels at +-value, the rest unit normal), "wrowmax" / "woutliers" (the same on the weight rows / 8 weight
+    channels).  Weights are N(0, 0.03^2) where not set otherwise.  Generated on the CPU: the GPU tests feed the same numbers."""
+    g = torch.Generator().manual_seed(seed + K)
+    a = torch.randn(rows, K, generator=g, dtype=torch.float64).float()
+    w = torch.randn(cols, K, generator=g, dtype=torch.float64).float() * 0.03
+    idx = torch.randperm(K, generator=g)[:8]
+    sign = lambda n: torch.randint(0, 2, (n, 8), generator=g).float() * 2 - 1
+    if kind == "rowmax":
+        a = a / a.abs().amax(1, keepdim=True) * value
+    elif kind == "outliers":
+        a[:, idx] = sign(rows) * value
+    elif kind == "wrowmax":
+        w = w / w.abs().amax(1, keepdim=True) * value
+    elif kind == "woutliers":
+        w[:, idx] = sign(cols) * value
+    else:
+        raise ValueError(kind)
+    return a, w
+
+
+def split_errors(a, w):
+    """max |C - A.W| / (|A|.|W|^T) of the split product (exact products, fp64 sums) and of the fp16 pass Ah.Wh alone."""
+    ah, a8 = split_planes(a)
+    wh, w8 = split_planes(w, weight=True)
+    e = lambda p: p.view(torch.float8_e4m3fn).double()
+    one = ah.double() @ wh.double().t()
+    split = one + (e(a8) @ e(w8).t()) * 2.0 ** -14
+    exact = a.double() @ w.double().t()
+    norm = a.double().abs() @ w.double().abs().t()
+    return ((split - exact).abs() / norm).max().item(), ((one - exact).abs() / norm).max().item()
+
+
+# (kind, value): inside the range
+IN_RANGE = [("rowmax", 448.0), ("rowmax", 4.0), ("rowmax", 1.0), ("rowmax", 2.0 ** -2), ("rowmax", 2.0 ** -4), ("wrowmax", 1.0),
+            ("wrowmax", 2.0 ** -6)]
+IN_RANGE_OUTLIERS = [("outliers", 300.0), ("outliers", 448.0), ("woutliers", 28.0)]
+# ... and outside it: activation outliers past 464, activation rows below 2^-6, weight channels past 28, weight rows below 2^-9
+OUT_OF_RANGE = [("outliers", 1000.0), ("outliers", 4000.0), ("rowmax", 2.0 ** -7), ("rowmax", 2.0 ** -8), ("woutliers", 40.0),
+                ("wrowmax", 2.0 ** -11)]
+
+
+@pytest.mark.parametrize("kind,value", IN_RANGE + IN_RANGE_OUTLIERS)
+@pytest.mark.parametrize("K", [1280, 5120])
+def test_split_accuracy_inside_the_range(kind, value, K):
+    err, err_one = split_errors(*range_case(kind, value, K))
+    bound = OUTLIER_BOUND if "outliers" in kind else RANGE_BOUND
+    assert err < bound and err < err_one / 6, (math.log2(err), math.log2(err_one))
+
+
+@pytest.mark.parametrize("kind,value", OUT_OF_RANGE)
+def test_split_accuracy_outside_the_range(kind, value):
+    """Past the range the class is lost (the error leaves OUTLIER_BOUND), but the result stays a correction of the fp16 pass."""
+    err, err_one = split_errors(*range_case(kind, value))
+    assert math.isfinite(err) and err <= err_one, (math.log2(err), math.log2(err_one))
+    assert err > OUTLIER_BOUND, math.log2(err)
+
+
+def test_slot_limits_of_the_split():
+    """Where the slots leave e4m3's normal range: slot 0 of an activation holds 416 exactly and saturates at 448 from there on
+    (464, the tie between 448 and the unrepresentable 480, rounds down to it); 2^10 Al of a row at 2^-7 is subnormal; slot 1 of a
+    weight saturates at |W| = 28."""
+    x = torch.tensor([[416.0, 448.0, 464.0, 465.0, 896.0, -1000.0] + [0.0] * 26])
+    _, p8 = split_planes(x)
+    assert p8.view(torch.float8_e4m3fn).float()[0, :6].tolist() == [416.0, 448.0, 448.0, 448.0, 448.0, -448.0]
+    g = torch.Generator().manual_seed(3)
+    row = 2.0 ** -7 * (1 + torch.rand(1, 32, generator=g))
+    _, p8 = split_planes(row)
+    slot1 = p8.view(torch.float8_e4m3fn).float()[0, 32:]
+    assert 0 < slot1.abs().max() < 2.0 ** -6                                               # e4m3's smallest normal
+    w = torch.tensor([[26.0, 28.0, 28.5, 40.0] + [0.0] * 28])
+    _, w8 = split_planes(w, weight=True)
+    assert w8.view(torch.float8_e4m3fn).float()[0, 32:36].tolist() == [416.0, 448.0, 448.0, 448.0]
 
 
 FORMATS = {"bf16": (torch.bfloat16, None), "bf16x2": (torch.bfloat16, torch.bfloat16), "f16": (torch.float16, None),
