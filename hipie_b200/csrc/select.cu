@@ -106,7 +106,16 @@ __device__ void bitonic_sort_desc(float* key, int* idx, int n2) {
     }
 }
 
-constexpr int NMS_MAX = 2048;     // boxes per image (HIPIE: 900)
+// shared memory of batched_nms_kernel for N boxes: sort keys and indices, offset boxes, the N x N pair bit matrix, removed bits
+constexpr int nms_smem_bytes(int N) {
+    int n2 = 4;
+    while (n2 < N) n2 <<= 1;
+    const int words = (N + 31) / 32;
+    return n2 * 8 + N * 16 + N * words * 4 + words * 4 + 64;
+}
+constexpr int NMS_SMEM_CAP = 220 * 1024;
+constexpr int NMS_MAX = 1216;     // boxes per image (HIPIE: 900): the largest N whose pair matrix fits NMS_SMEM_CAP
+static_assert(nms_smem_bytes(NMS_MAX) <= NMS_SMEM_CAP && nms_smem_bytes(NMS_MAX + 1) > NMS_SMEM_CAP, "NMS_MAX is the shared-memory limit");
 
 // boxes (B, N, 4) cxcywh normalised | scores (B, N) | cls (B, N) int32 -> keep (B, N) int32 kept indices in decreasing score
 // order (-1 padded), nkeep (B)
@@ -150,7 +159,9 @@ __global__ void __launch_bounds__(1024) batched_nms_kernel(const float* __restri
     for (int i = threadIdx.x; i < N; i += blockDim.x) {
         const int s = idx[i];
         const float cx = bb[4 * s], cy = bb[4 * s + 1], w = bb[4 * s + 2], h = bb[4 * s + 3];
-        const float o = (float)cls[(size_t)b * N + s] * off1;            // offsets = idxs.to(boxes) * (max_coordinate + 1)
+        // offsets = idxs.to(boxes) * (max_coordinate + 1), rounded before the add as torchvision's tensors are: a contracted
+        // cls * off1 + x (one FMA) moves the boxes of class ids in the hundreds by up to 6e-5 at coordinates ~1700
+        const float o = __fmul_rn((float)cls[(size_t)b * N + s], off1);
         bx[i] = make_float4((cx - 0.5f * w) + o, (cy - 0.5f * h) + o, (cx + 0.5f * w) + o, (cy + 0.5f * h) + o);
     }
     for (int i = threadIdx.x; i < words; i += blockDim.x) removed[i] = 0;
@@ -160,7 +171,7 @@ __global__ void __launch_bounds__(1024) batched_nms_kernel(const float* __restri
         const int i = t / words, wj = t - i * words;
         uint32_t m = 0;
         const float4 a = bx[i];
-        const float sa = (a.z - a.x) * (a.w - a.y);
+        const float sa = __fmul_rn(a.z - a.x, a.w - a.y);      // areas and intersection rounded as torchvision's (no FMA into the sum)
         const int j0 = wj * 32;
         if (j0 + 31 > i) {
             for (int jj = 0; jj < 32; ++jj) {
@@ -170,8 +181,8 @@ __global__ void __launch_bounds__(1024) batched_nms_kernel(const float* __restri
                     const float left = fmaxf(a.x, c.x), right = fminf(a.z, c.z);
                     const float top = fmaxf(a.y, c.y), bottom = fminf(a.w, c.w);
                     const float width = fmaxf(right - left, 0.f), height = fmaxf(bottom - top, 0.f);
-                    const float inter = width * height;
-                    const float sb = (c.z - c.x) * (c.w - c.y);
+                    const float inter = __fmul_rn(width, height);
+                    const float sb = __fmul_rn(c.z - c.x, c.w - c.y);
                     if (inter / (sa + sb - inter) > thr) m |= 1u << jj;
                 }
             }
@@ -379,11 +390,7 @@ extern "C" int hipie_batched_nms(const float* boxes_cxcywh, const float* scores,
     HIPIE_CHECK_ARG(boxes_cxcywh && scores && cls && keep && nkeep, "hipie_batched_nms: null pointer argument");
     HIPIE_CHECK_ARG(B >= 0 && N > 0 && N <= NMS_MAX, "hipie_batched_nms: N=%d outside (0, %d]", N, NMS_MAX);
     if (B == 0) return HIPIE_OK;
-    int n2 = 4;
-    while (n2 < N) n2 <<= 1;
-    const int words = (N + 31) / 32;
-    const int smem = n2 * 8 + N * 16 + N * words * 4 + words * 4 + 64;
-    HIPIE_CHECK_ARG(smem <= 220 * 1024, "hipie_batched_nms: N=%d needs %d B of shared memory", N, smem);
+    const int smem = nms_smem_bytes(N);
     HIPIE_ENSURE_SMEM(batched_nms_kernel, smem);
     batched_nms_kernel<<<B, 1024, smem, (cudaStream_t)stream>>>(boxes_cxcywh, scores, cls, keep, nkeep, N, iou_threshold);
     HIPIE_CHECK_LAUNCH();

@@ -318,7 +318,7 @@ int hipie_class_scores(const float* logits, const int* tok, const int* cnt, cons
 /* hipie_batched_nms: torchvision.ops.batched_nms semantics (coordinate-offset trick: box + cls * (max_coord + 1), greedy in
  * decreasing score, IoU = inter / (a + b - inter) > threshold), one launch for B images.
  *   boxes (B, N, 4) f32 (cx, cy, w, h) | scores (B, N) f32 | cls (B, N) i32
- *   keep (B, N) i32 out: kept indices in decreasing score order, -1 padded | nkeep (B) i32 out.  N <= ~1300. */
+ *   keep (B, N) i32 out: kept indices in decreasing score order, -1 padded | nkeep (B) i32 out.  N <= 1216 (the pair bit matrix lives in shared memory). */
 int hipie_batched_nms(const float* boxes_cxcywh, const float* scores, const int* cls, int* keep, int* nkeep, int B, int N,
                       float iou_threshold, void* stream);
 
