@@ -37,6 +37,11 @@ __device__ __forceinline__ float rcp_approx(float x) {
     return y;
 }
 
+// A low-resolution logit as staged: -log2(e) * logit, rounded on its own.  __fmul_rn, because the recomputation of the
+// winner's sigmoid after the argmax must see the value the loop read from shared memory, and a plain product there could
+// be contracted into the following subtraction.
+__device__ __forceinline__ float stage_tap(float logit) { return __fmul_rn(-1.4426950408889634f, logit); }
+
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
 }
@@ -47,6 +52,12 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
 //
 // masks (Q,h,w) f32 | pt_hi/pt_lo (NT*8, Qpad) bf16 = class probabilities transposed, split | scores (Qpad) f32, 0 = not kept
 // sem (C,Hc,Wc) f32 | ids (Hc,Wc) i32 = -1 or 2*q + (sigmoid_q >= .5) | areas (3,Q) i32 = mask / original / intersection
+//
+// The original-area count, the winner's intersection bit and the argmax all read one sigmoid value per (pixel, query), and
+// "inside the mask" is `s >= 0.5f` on it, as the reference's fp32 `sigmoid >= 0.5`.  That predicate is not `logit >= 0`: fp32
+// rounds 1 + exp(-x) to 2 for logits down to about -1.8e-7, and the panoptic merge needs intersection <= original exactly.
+// The winner's bit is recomputed after the argmax from the same four taps by the same instructions, so it is the value the
+// count read; it is never re-derived from the product score * sigmoid, which can round onto 0.5 * score.
 template <int NT>
 __global__ void __launch_bounds__(PP_THREADS, NT <= 10 ? 2 : 1)
 seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict__ pt_hi,
@@ -88,7 +99,7 @@ seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict
         for (int k = 0; k < PP_NLD; ++k) {
             const int ql = (tid + k * PP_THREADS) / PP_TQ;
             // staged as -log2(e) * logit, so sigmoid = 1 / (1 + 2^tap); padding -> +big -> sigmoid 0
-            tv[k] = (goff[k] >= 0 && q0 + ql < Q) ? -1.4426950408889634f * __ldg(masks + (size_t)q0 * hw + goff[k]) : 1e30f;
+            tv[k] = (goff[k] >= 0 && q0 + ql < Q) ? stage_tap(__ldg(masks + (size_t)q0 * hw + goff[k])) : 1e30f;
         }
     };
     auto store_taps = [&](int buf) {
@@ -191,7 +202,7 @@ seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict
                             const bool up = pr > best[ps];
                             best[ps] = up ? pr : best[ps];
                             bidx[ps] = up ? q0 + ql : bidx[ps];
-                            n += (pv[ps] && v <= 0.f) ? 1u : 0u;                    // sigmoid >= .5  <=>  logit >= 0
+                            n += (pv[ps] && s >= 0.5f) ? 1u : 0u;
                         }
                     }
                     npack |= n << (8 * j);
@@ -227,7 +238,26 @@ seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict
     }
 
     // ---- argmax across the quad (ties -> lowest query index, like torch.argmax over the kept list) -------------
-    // A pixel where every kept query has score*sigmoid == 0 (sigmoid underflow) goes to the first kept query, as argmax would.
+    // A pixel where every kept query has score*sigmoid == 0 (sigmoid underflow) goes to the first kept query, as argmax would,
+    // with the bit 0: its sigmoid is 0 there (rcp.approx.ftz has no denormal results).
+    // sigmoid of query q at pixel ps, bit for bit the loop's value: the same rounded taps (stage_tap keeps the product out of
+    // any fma), the same explicit fma / add sequence and the same approximations
+    auto sigmoid_at = [&](int q, int ps) {
+        const int mt = ps >> 1, kxl = 2 * (warp & 3) + mt;
+        const float* mq = masks + (size_t)q * hw;
+        float tt[2][2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int yy = min(max(y_lo + kyl + r, 0), h - 1), xx = min(max(x_lo + kxl + c, 0), w - 1);
+                tt[r][c] = stage_tap(__ldg(mq + (size_t)yy * w + xx));
+            }
+        const float top = fmaf(lx1, tt[0][1] - tt[0][0], tt[0][0]);
+        const float bot = fmaf(lx1, tt[1][1] - tt[1][0], tt[1][0]);
+        const float v = fmaf((ps & 1) ? lyb1 : lya1, bot - top, top);
+        return rcp_approx(1.f + ex2_approx(v));
+    };
 #pragma unroll
     for (int ps = 0; ps < 4; ++ps) {
 #pragma unroll
@@ -243,7 +273,7 @@ seg_post_kernel(const float* __restrict__ masks, const __nv_bfloat16* __restrict
         if (t == 0 && pv[ps]) {
             const int y = (ps & 1) ? y_b : y_a;
             int bi = bidx[ps], in = 0;
-            if (bi >= 0) in = best[ps] >= 0.5f * scores[bi];      // sigmoid >= .5 for the winner
+            if (bi >= 0) in = sigmoid_at(bi, ps) >= 0.5f;
             else bi = s_first == 0x7fffffff ? -1 : s_first;
             ids[(size_t)y * Wc + px[ps >> 1]] = bi < 0 ? -1 : 2 * bi + in;
             if (bi >= 0) {
