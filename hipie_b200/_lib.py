@@ -108,6 +108,10 @@ SYMBOLS = {
     "hipie_sam_vote": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p] + [c_int] * 4 + [c_void_p] * 5),
     "hipie_semseg_confusion": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 3),
     "hipie_panoptic_pairs": (c_int, [c_void_p] * 2 + [c_int] * 2 + [c_void_p] + [c_int] * 2 + [c_void_p] * 3),
+    "hipie_mask_words": (c_int64, [c_int, c_int]),
+    "hipie_mask_pack": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p] * 3),
+    "hipie_rle_expand": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p] * 3),
+    "hipie_mask_overlaps": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 3 + [c_void_p] * 2),
 }
 
 

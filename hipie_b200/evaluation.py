@@ -9,6 +9,8 @@ image's pair table (a few KB) is copied asynchronously into pinned memory and ma
 are computed from those counters exactly as the reference computes them, quirks included (DESIGN.md, "Evaluation").
 
     SemSegEvaluator / COCOPanopticEvaluator   reset() / process(inputs, outputs) / evaluate(), the reference's DatasetEvaluator surface
+    COCOInstanceEvaluator                     AP_bbox / AP_segm (COCOEvaluator / InstanceSegEvaluator): mask overlaps on the device,
+                                              COCOeval's matching on the host (cocoeval.py)
     PRESETS, load_records                     readers for the reference's dataset layouts under a data root
     preset_vocabulary                         the test mapper's vocabulary of a preset (coco_dataset_mapper_uni.py:196-215, 556-566)
     evaluate_dataset                          the eval-only driver; `python -m hipie_b200.evaluation` is its command line
@@ -17,13 +19,14 @@ import argparse
 import collections
 import json
 import os
+import sys
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import cocoeval, ops
 from .data import ResizeShortestEdge, create_queries_and_maps, get_openseg_labels
 from .hostio import PinnedArena
 from .parallel import shard_indices
@@ -374,6 +377,126 @@ class COCOPanopticEvaluator:
         return {"panoptic_seg": res, "panoptic_seg_per_class": per_class}
 
 
+class COCOInstanceEvaluator:
+    """detectron2's COCOEvaluator / InstanceSegEvaluator (bbox and segm) with the mask overlaps on the device.  instances_json: the
+    dataset's COCO instance annotations; thing_dataset_id_to_contiguous_id maps the model's classes back to dataset ids (a class outside
+    it raises, as the reference's assert does); class_names: the AP-<name> keys, one per instance category (the reference asserts that
+    count in _derive_coco_results).
+
+    process() packs the predicted masks (ops.mask_pack), expands the image's GT runs (ops.rle_expand), launches ops.mask_overlaps and
+    copies the (N, M) intersection table, the mask areas, boxes, scores and classes into pinned memory.  Once the copy has landed (a
+    later process() call or evaluate()) COCOeval.evaluateImg runs for both tasks and only its compact per-image records are kept.
+    evaluate() gathers the records to rank 0 and accumulates them in image-id order.  Only processed images count."""
+
+    TASKS = ("bbox", "segm")
+
+    def __init__(self, instances_json, thing_dataset_id_to_contiguous_id, class_names, distributed=True):
+        with open(instances_json, "r") as f:
+            js = json.load(f)
+        self.cat_ids = sorted(c["id"] for c in js["categories"])
+        self.class_names = list(class_names)
+        if len(self.class_names) != len(self.cat_ids):
+            raise ValueError(f"COCOInstanceEvaluator: {len(self.class_names)} thing classes for the {len(self.cat_ids)} categories of "
+                             f"{instances_json}")
+        self.images = {im["id"]: im for im in js["images"]}
+        self._by_stem = {os.path.splitext(os.path.basename(im["file_name"]))[0]: im["id"] for im in js["images"]}
+        self.anns = collections.defaultdict(list)
+        for a in js["annotations"]:
+            self.anns[a["image_id"]].append(a)
+        self._dataset_id = {v: k for k, v in thing_dataset_id_to_contiguous_id.items()}
+        self._distributed = distributed
+        self._stage = _Inflight()
+        self.reset()
+
+    def reset(self):
+        self._records = []                 # (image id, {task: image_records})
+        self._any_predictions = False
+
+    def _image_id(self, inp):
+        if inp["image_id"] in self.images:
+            return inp["image_id"]
+        stem = os.path.splitext(os.path.basename(inp.get("file_name", "")))[0]
+        if stem in self._by_stem:
+            return self._by_stem[stem]
+        raise KeyError(f"COCOInstanceEvaluator: image {inp['image_id']} is not in the instance annotations")
+
+    def process(self, inputs, outputs):
+        for inp, out in zip(inputs, outputs):
+            inst = out["instances"]
+            img_id = self._image_id(inp)
+            H, W = self.images[img_id]["height"], self.images[img_id]["width"]
+            masks = inst.pred_masks
+            if masks.dim() != 3 or tuple(masks.shape[1:]) != (H, W):
+                raise ValueError(f"COCOInstanceEvaluator: masks of image {inp['image_id']} are {tuple(masks.shape)}, the image {H} x {W}")
+            anns = self.anns.get(img_id, [])
+            runs = [cocoeval.ann_to_runs(a, H, W) for a in anns]
+            gts = [{"id": a["id"], "category_id": a["category_id"], "iscrowd": a.get("iscrowd", 0), "area": a["area"]} for a in anns]
+            gt_pixels = [cocoeval.runs_area(r) for r in runs]
+            gt_boxes = [a["bbox"] for a in anns]
+            N, M = masks.shape[0], len(runs)
+            dev = masks.device
+            arena = self._stage.acquire()
+            err = torch.zeros(1, dtype=torch.int64, device=dev)
+            pbits, parea = ops.mask_pack(masks)
+            if N and M:
+                ends, offsets = ops.rle_ends(runs, H, W)
+                gbits = ops.rle_expand(arena.to_device(ends, dev), arena.to_device(offsets, dev), H, W, err=err)
+            else:
+                gbits = torch.zeros((M, ops.mask_words(H, W)), dtype=torch.int32, device=dev)
+            inter = ops.mask_overlaps(pbits, gbits, H, W)
+            host = [arena.to_host(t) for t in (inter, parea, inst.pred_boxes.tensor.float(), inst.scores.float(),
+                                               inst.pred_classes.to(torch.int64), err)]
+            image_id = inp["image_id"]
+
+            def done(host=host, gts=gts, gt_pixels=gt_pixels, gt_boxes=gt_boxes, img_id=img_id, image_id=image_id):
+                inter_h, area_h, boxes_h, scores_h, classes_h, err_h = (t.numpy() for t in host)
+                if int(err_h[0]):
+                    raise ValueError(f"COCOInstanceEvaluator: GT run lists of image {image_id} do not cover the image")
+                self._add_image(img_id, inter_h, area_h, boxes_h, scores_h, classes_h, gts, gt_pixels, gt_boxes)
+
+            self._stage.release(arena, done)
+
+    def _add_image(self, img_id, inter, area, boxes, scores, classes, gts, gt_pixels, gt_boxes):
+        """instances_to_coco_json + COCOeval.evaluateImg of one image: XYXY -> XYWH in float32 (BoxMode.convert), then Python floats."""
+        for c in classes.tolist():
+            if c not in self._dataset_id:
+                raise ValueError(f"A prediction has class={c}, but the dataset only has class ids in "
+                                 f"{sorted(self._dataset_id)} (thing_dataset_id_to_contiguous_id).")
+        xywh = boxes.astype(np.float32).copy()
+        xywh[:, 2] -= xywh[:, 0]
+        xywh[:, 3] -= xywh[:, 1]
+        xywh = xywh.tolist()
+        scores = scores.tolist()
+        cats = [self._dataset_id[c] for c in classes.tolist()]
+        crowd = [g["iscrowd"] for g in gts]
+        recs = {}
+        for task in self.TASKS:
+            if task == "segm":
+                dts = [{"category_id": c, "score": s, "area": int(a)} for c, s, a in zip(cats, scores, area.tolist())]
+                ious = cocoeval.mask_iou(inter, area, gt_pixels, crowd)
+            else:
+                dts = [{"category_id": c, "score": s, "area": b[2] * b[3]} for c, s, b in zip(cats, scores, xywh)]
+                ious = cocoeval.bbox_iou(xywh, gt_boxes, crowd)
+            recs[task] = cocoeval.image_records(self.cat_ids, gts, dts, ious)
+        self._records.append((img_id, recs))
+        self._any_predictions = self._any_predictions or len(scores) > 0
+
+    def evaluate(self):
+        self._stage.drain()
+        records, any_pred = self._records, self._any_predictions
+        if self._distributed and _distributed():
+            parts = [None] * dist.get_world_size() if dist.get_rank() == 0 else None
+            dist.gather_object((records, any_pred), parts, dst=0)
+            if dist.get_rank() != 0:
+                return None
+            records = [r for p in parts for r in p[0]]
+            any_pred = any(p[1] for p in parts)
+        res = collections.OrderedDict()
+        for task in self.TASKS:
+            res[task] = cocoeval.evaluate_records([(i, r[task]) for i, r in records], self.cat_ids, self.class_names, any_pred)
+        return res
+
+
 # ---------------------------------------------------------------------------------------------------------------------------------
 # datasets
 
@@ -393,10 +516,12 @@ PRESETS = {
     "ade20k_panoptic_val": dict(
         kind="panoptic", vocabulary="ade20k_150", ignore_label=255, image_root="ade/ADEChallengeData2016/images/validation",
         panoptic_root="ade/ADEChallengeData2016/ade20k_panoptic_val", panoptic_json="ade/ADEChallengeData2016/ade20k_panoptic_val.json",
-        sem_seg_root="ade/ADEChallengeData2016/annotations_detectron2/validation"),
+        sem_seg_root="ade/ADEChallengeData2016/annotations_detectron2/validation",
+        instances_json="ade/ADEChallengeData2016/ade20k_instance_val.json"),
     "coco_2017_val_panoptic_with_sem_seg": dict(
         kind="panoptic", vocabulary="coco_panoptic", ignore_label=255, image_root="coco/val2017", panoptic_root="coco/panoptic_val2017",
-        panoptic_json="coco/annotations/panoptic_val2017.json", sem_seg_root="coco/panoptic_semseg_val2017"),
+        panoptic_json="coco/annotations/panoptic_val2017.json", sem_seg_root="coco/panoptic_semseg_val2017",
+        instances_json="coco/annotations/instances_val2017.json"),
     "ade20k_full_sem_seg_val": dict(
         kind="sem_seg", vocabulary="ade20k_847", ignore_label=65535, num_classes=847,
         image_root="ade/ADE20K_2021_17_01/images_detectron2/validation", sem_seg_root="ade/ADE20K_2021_17_01/annotations_detectron2/validation",
@@ -480,7 +605,8 @@ def load_panoptic_json(json_file, image_dir, gt_dir, semseg_dir):
 
 def load_records(name, root=None):
     """-> (records, metadata) of a preset under the data root.  metadata: ignore_label, class_names, num_classes, vocabulary, and for
-    panoptic presets panoptic_json / panoptic_root / categories / the contiguous-id maps."""
+    panoptic presets panoptic_json / panoptic_root / categories / the contiguous-id maps / instances_json (the COCO instance
+    annotations, which may be absent)."""
     p = preset(name)
     paths = _paths(name, data_root(root))
     meta = {"name": name, "ignore_label": p["ignore_label"], "vocabulary": p["vocabulary"]}
@@ -490,6 +616,8 @@ def load_records(name, root=None):
         meta.update(panoptic_json=paths["panoptic_json"], panoptic_root=paths["panoptic_root"], categories=cats,
                     thing_dataset_id_to_contiguous_id=things, stuff_dataset_id_to_contiguous_id=stuff,
                     class_names=[c["name"] for c in cats], num_classes=len(cats))
+        if "instances_json" in paths:
+            meta["instances_json"] = paths["instances_json"]
     else:
         records = load_sem_seg(paths["sem_seg_root"], paths["image_root"], gt_ext=p["gt_ext"], image_ext=p["image_ext"])
         meta.update(thing_dataset_id_to_contiguous_id={}, num_classes=p["num_classes"], class_names=None)
@@ -512,7 +640,9 @@ def preset_vocabulary(name, tokenizer, labels_root=None, thing_contiguous_ids=()
 
 
 def default_evaluators(meta, records, labels_root=None):
-    """SemSegEvaluator (every preset) and COCOPanopticEvaluator (panoptic presets), as the reference's build_evaluator picks them."""
+    """SemSegEvaluator (every preset), COCOPanopticEvaluator (panoptic presets) and COCOInstanceEvaluator (panoptic presets whose
+    instance JSON exists), as the reference's build_evaluator picks them.  A missing instance JSON leaves the other two as they are and
+    says so in one line on stderr."""
     names = meta["class_names"]
     if names is None:
         names = [c["name"] for c in get_openseg_labels(meta["vocabulary"], root=labels_root)]
@@ -522,6 +652,13 @@ def default_evaluators(meta, records, labels_root=None):
     if "panoptic_json" in meta:
         evs.insert(0, COCOPanopticEvaluator(meta["panoptic_json"], meta["panoptic_root"], meta["thing_dataset_id_to_contiguous_id"],
                                             meta["stuff_dataset_id_to_contiguous_id"]))
+    inst = meta.get("instances_json")
+    if inst is not None:
+        if os.path.isfile(inst):
+            things = [c["name"] for c in meta["categories"] if c.get("isthing", 0)]
+            evs.insert(0, COCOInstanceEvaluator(inst, meta["thing_dataset_id_to_contiguous_id"], things))
+        else:
+            print(f"{meta['name']}: instance annotations {inst} not found; AP_bbox / AP_segm are not evaluated", file=sys.stderr)
     return evs
 
 
@@ -611,7 +748,8 @@ def _json_safe(o):
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="Evaluate HIPIE on a segmentation benchmark (mIoU, and PQ on panoptic presets).")
+    ap = argparse.ArgumentParser(description="Evaluate HIPIE on a segmentation benchmark (mIoU; PQ, and AP_bbox / AP_segm when the "
+                                             "instance JSON is present, on panoptic presets).")
     ap.add_argument("--config-file", required=True)
     ap.add_argument("--dataset", required=True, choices=sorted(PRESETS))
     ap.add_argument("--data-root", default=None)

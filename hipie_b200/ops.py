@@ -7,6 +7,7 @@ here computes on the CPU or through ATen; a missing library or a CPU tensor rais
 import ctypes
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1067,3 +1068,95 @@ def panoptic_pairs(pred, gt_rgb, gt_ids, S, err=None):
     if check:
         _raise_on_errors(err, "panoptic_pairs", f"carry a predicted segment id outside 0..{S}")
     return table
+
+
+# ---- instance mask overlaps (COCO AP_segm): one bit layout for predictions and GTs, owned here and by hipie_mask_words
+MASK_MAX_PRED, MASK_MAX_GT = 1024, 4096
+
+
+def mask_words(H, W):
+    """u32 words per packed mask: the row-major pixels of an H x W mask, 32 per word, zero-padded to whole 256-bit chunks."""
+    return (int(H) * int(W) + 255) // 256 * 8
+
+
+def _check_hw(what, H, W):
+    if not (H > 0 and W > 0 and H * W < (1 << 31)):
+        raise ValueError(f"{what}: bad image size {H} x {W} (H * W < 2^31)")
+
+
+def mask_pack(masks):
+    """hipie_mask_pack: masks (N, H, W) uint8 / bool -> (bits (N, mask_words(H, W)) int32, area (N,) int32 pixel counts).  N <= 1024;
+    N = 0 returns empty tensors without a launch."""
+    masks = masks.contiguous()
+    if masks.dtype == torch.bool:
+        masks = masks.view(torch.uint8)
+    if masks.dim() != 3 or masks.dtype != torch.uint8:
+        raise ValueError(f"mask_pack: masks must be (N, H, W) uint8, got {tuple(masks.shape)} {masks.dtype}")
+    N, H, W = masks.shape
+    _check_hw("mask_pack", H, W)
+    if N > MASK_MAX_PRED:
+        raise ValueError(f"mask_pack: {N} masks (at most {MASK_MAX_PRED})")
+    bits = torch.empty((N, mask_words(H, W)), dtype=torch.int32, device=masks.device)
+    area = torch.zeros(N, dtype=torch.int32, device=masks.device)
+    if N:
+        with _timed("mask_pack", float(masks.numel())):
+            _lib.check(_lib.load().hipie_mask_pack(_p(masks), N, H, W, _p(bits), _p(area), _stream()), "mask_pack")
+    return bits, area
+
+
+def rle_ends(runs, H, W):
+    """Host side of rle_expand: a sequence of COCO run-length lists (column-major counts, background first) -> (ends int32, offsets
+    int64 (M + 1)) numpy arrays, the cumulative run ends of every list back to back.  A list with a negative count or not summing to
+    H * W raises."""
+    _check_hw("rle_ends", H, W)
+    if len(runs) > MASK_MAX_GT:
+        raise ValueError(f"rle_ends: {len(runs)} GT masks (at most {MASK_MAX_GT})")
+    ends, offsets = [], [0]
+    for i, r in enumerate(runs):
+        r = np.asarray(r, dtype=np.int64).reshape(-1)
+        e = np.cumsum(r)
+        if (r < 0).any() or not len(e) or e[-1] != H * W:
+            raise ValueError(f"rle_ends: run list {i} sums to {int(e[-1]) if len(e) else 0}, the image has {H} x {W} = {H * W} pixels")
+        ends.append(e.astype(np.int32))
+        offsets.append(offsets[-1] + len(e))
+    return (np.concatenate(ends) if ends else np.zeros(0, np.int32)), np.asarray(offsets, dtype=np.int64)
+
+
+def rle_expand(ends, offsets, H, W, err=None):
+    """hipie_rle_expand: device ends (int32) / offsets (int64, M + 1) from rle_ends -> bits (M, mask_words(H, W)) int32.  Lists whose
+    last end is not H * W are counted in err (as semseg_confusion); without err the call waits and raises on them.  M <= 4096; M = 0
+    returns an empty tensor without a launch."""
+    _check_hw("rle_expand", H, W)
+    if offsets.dtype != torch.int64 or offsets.dim() != 1 or ends.dtype != torch.int32 or ends.dim() != 1:
+        raise ValueError("rle_expand: ends must be 1-D int32 and offsets 1-D int64")
+    M = offsets.numel() - 1
+    if not 0 <= M <= MASK_MAX_GT:
+        raise ValueError(f"rle_expand: {M} GT masks (at most {MASK_MAX_GT})")
+    bits = torch.empty((M, mask_words(H, W)), dtype=torch.int32, device=ends.device)
+    if M == 0:
+        return bits
+    err, check = _error_counter(err, ends.device, "rle_expand")
+    ends, offsets = ends.contiguous(), offsets.contiguous()
+    with _timed("rle_expand", float(bits.numel() * 4)):
+        _lib.check(_lib.load().hipie_rle_expand(_p(ends), _p(offsets), M, H, W, _p(bits), _p(err), _stream()), "rle_expand")
+    if check and int(err.item()):
+        raise ValueError(f"rle_expand: {int(err.item())} run lists do not sum to {H} x {W} = {H * W} pixels")
+    return bits
+
+
+def mask_overlaps(pred_bits, gt_bits, H, W):
+    """hipie_mask_overlaps: pred_bits (N, KW) and gt_bits (M, KW) int32 from mask_pack / rle_expand -> inter (N, M) int32 pixel counts of
+    every pair's intersection (b1 MMA, K split over CTAs, exact).  N = 0 or M = 0 returns an empty table without a launch."""
+    _check_hw("mask_overlaps", H, W)
+    KW = mask_words(H, W)
+    for name, t, lim in (("pred_bits", pred_bits, MASK_MAX_PRED), ("gt_bits", gt_bits, MASK_MAX_GT)):
+        if t.dtype != torch.int32 or t.dim() != 2 or t.shape[1] != KW or not t.is_contiguous():
+            raise ValueError(f"mask_overlaps: {name} must be contiguous (rows, {KW}) int32, got {tuple(t.shape)} {t.dtype}")
+        if t.shape[0] > lim:
+            raise ValueError(f"mask_overlaps: {t.shape[0]} rows of {name} (at most {lim})")
+    N, M = pred_bits.shape[0], gt_bits.shape[0]
+    inter = torch.zeros((N, M), dtype=torch.int32, device=pred_bits.device)
+    if N and M:
+        with _timed("mask_overlaps", float((N + M) * KW * 4)):
+            _lib.check(_lib.load().hipie_mask_overlaps(_p(pred_bits), N, _p(gt_bits), M, H, W, _p(inter), _stream()), "mask_overlaps")
+    return inter

@@ -452,6 +452,18 @@ int hipie_semseg_confusion(const float* sem, int C, int H, int W, const int* gt,
 int hipie_panoptic_pairs(const int* pred, const uint8_t* gt_rgb, int H, int W, const int* gt_ids, int n_gt, int S,
                          unsigned long long* table, unsigned long long* err, void* stream);
 
+/* ---- instance mask overlaps (pycocotools maskApi.c rleIou on the RLEs of detectron2's COCOEvaluator).  One bit layout: a mask is its
+ * row-major pixels (bit j of word w = pixel y * W + x = 32 w + j), zero-padded to whole 256-bit chunks, KW = hipie_mask_words(H, W) u32
+ * words per mask.  N <= 1024 predictions, M <= 4096 GTs, H * W < 2^31; N = 0 / M = 0 launch nothing.  No call synchronises.
+ * hipie_mask_pack: masks (N, H, W) uint8 (non-zero = inside) -> bits (N, KW), area[n] += pixel count (i32, zeroed by the caller).
+ * hipie_rle_expand: GT g's column-major COCO runs (background first) as cumulative ends ends[offsets[g] .. offsets[g + 1]) (i32, offsets
+ *   (M + 1) i64) -> bits (M, KW).  A list whose last end is not H * W is counted in *err (u64, accumulated).
+ * hipie_mask_overlaps: inter (N, M) i32 (zeroed by the caller) += sum_k popc(pred_bits[n, k] & gt_bits[m, k]). */
+int64_t hipie_mask_words(int H, int W);
+int hipie_mask_pack(const uint8_t* masks, int N, int H, int W, uint32_t* bits, int* area, void* stream);
+int hipie_rle_expand(const int* ends, const int64_t* offsets, int M, int H, int W, uint32_t* bits, unsigned long long* err, void* stream);
+int hipie_mask_overlaps(const uint32_t* pred_bits, int N, const uint32_t* gt_bits, int M, int H, int W, int* inter, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
